@@ -240,9 +240,9 @@ struct TileChoice {
 // FLOP / clk / SM): the wgmma main loop of a 128 x BN tile takes k-blocks x (4 BN + 96) clk (tensor-core time plus the
 // per-k-block barrier and issue overhead), the register epilogue BN x {20 plain / RoPE, 24 reduce-add, 32 GELU} clk.
 // Tiles run in rounds over the SMs; the producer streams the next tile's operands during the epilogue, so a round
-// costs main + epilogue.  Checked against the graph-timed sweep of tools/gemm_sweep.py (H100 SXM 80 GB, 400 W power
-// limit) at M = 1876 and 15008: the pick is the fastest width or within 10 % of it.  Cluster pairs (cta_pair = 1) were
-// 1.3 - 2x slower than single-CTA tiles in every row of that sweep, so the planner never picks them.
+// costs main + epilogue.  Checked against the graph-timed sweep of tools/gemm_sweep.py with the chunked epilogue (H100
+// SXM 80 GB, 700 W limit): the pick is the fastest width at M = 1876 and within 11 % of it at M = 3752 - 15008.  Cluster
+// pairs (cta_pair = 1) were 1.6 - 3.8x slower than single-CTA tiles in every row of that sweep, so they are never picked.
 // Diagnostic build (make TRACE=1) only: F5_BN_<n_out>=<bn>[p] overrides the choice.
 TileChoice pick_tile(long long rows, int batches, int n_out, int k, int epi, int act) {
 #ifdef F5_TRACE
@@ -326,6 +326,12 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
   p.skip_pad = (a->skip_padded_tiles && a->row_len != nullptr && a->seq > 0 && (conv || a->batches == 1)) ? 1 : 0;
   // a prefetched W tile belongs to the CTA's first tile: not known to be computed when padded tiles are skipped
   p.w_prefetch = (a->weights_static && !p.skip_pad) ? 1 : 0;
+#ifdef F5_TRACE  // diagnostic build only: F5_GEMM_EPI=none runs the main loop without the epilogue
+  {
+    const char* e = getenv("F5_GEMM_EPI");
+    p.diag_no_epi = (e && strcmp(e, "none") == 0) ? 1 : 0;
+  }
+#endif
   int rc;
   if (conv) {
     if (a->n_out % 64 || a->lda < a->n_out) {

@@ -53,91 +53,153 @@ __device__ __forceinline__ bool tile_is_padding(const GemmParams& p, int m0, int
   return m0 - b0 * p.seq >= p.row_len[b0];
 }
 
-// fused epilogue of one row of the accumulator fragment: v[2 j], v[2 j + 1] are columns n0 + 8 j + c2, + 1
+// Fused epilogue of one thread's accumulator fragment: rows row0 and row0 + 8 (half h = 0, 1), columns
+// n0 + 8 j + c2 (+ 1) in acc[4 j + 2 h] (+ 1).  It runs over chunks of 8 to 64 columns, and every global load of a
+// chunk (bias, gate, RoPE cos / sin, residual) is issued before the first store of the chunk.  Stores may alias those
+// inputs as far as the compiler knows, so a loop that loads and stores per column pair waits one full memory latency
+// per pair; here a chunk waits about once.
 template <int BN, int EPI, int ACT>
-__device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* acc, int half, int n0, int c2,
-                                             int row_in_batch, int bz, const float* gate) {
-  if (row_in_batch >= p.rows) return;
-  const long long grow = (long long)bz * p.rows + row_in_batch;
-  bool valid = true;
-  int pos = 0;
-  if (p.seq > 0) {
-    pos = int(grow % p.seq);
-    if (p.row_len != nullptr) valid = pos < p.row_len[grow / p.seq];
-  }
-  if (EPI == EPI_RESID && !valid) return;
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* acc, int n0, int c2, int row0, int bz,
+                                              const float* gate) {
+  // chunk width: the widest whose loads fit beside the BN / 2 accumulators without spilling (ptxas caps a 288-thread
+  // CTA at 168 registers per thread)
+  constexpr int CW = BN <= 128 ? (EPI == EPI_QKV_ROPE ? 32 : 64)
+                     : BN == 192 ? (EPI == EPI_QKV_ROPE ? 16 : 32)
+                                 : (EPI == EPI_F16 ? 32 : EPI == EPI_RESID ? 16 : 8);
+  constexpr int J = CW / 8;  // column pairs of one thread in a chunk
+  bool in[2], valid[2];
+  long long grow[2];
+  int pos[2];
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int nc = n0 + 8 * j + c2;
-    if (nc >= p.n_out) continue;
-    const bool pair_ok = nc + 1 < p.n_out;
-    float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
-    if (p.bias != nullptr) {
-      if (pair_ok) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
-        v0 += b.x;
-        v1 += b.y;
-      } else {
-        v0 += __ldg(p.bias + nc);
+  for (int h = 0; h < 2; ++h) {
+    const int r = row0 + 8 * h;
+    in[h] = r < p.rows;
+    grow[h] = (long long)bz * p.rows + r;
+    valid[h] = true;
+    pos[h] = 0;
+    if (in[h] && p.seq > 0) {
+      pos[h] = int(grow[h] % p.seq);
+      if (p.row_len != nullptr) valid[h] = pos[h] < p.row_len[grow[h] / p.seq];
+    }
+    if (EPI == EPI_RESID) in[h] = in[h] && valid[h];  // masked rows keep their residual
+  }
+  if (!in[0] && !in[1]) return;
+#pragma unroll
+  for (int cc = 0; cc < BN / CW; ++cc) {
+    const int nb = n0 + CW * cc;
+    if (nb >= p.n_out) break;
+    // ---- loads ----
+    float2 b[J], g[J];
+#pragma unroll
+    for (int j = 0; j < J; ++j) {
+      const int nc = nb + 8 * j + c2;
+      b[j] = make_float2(0.0f, 0.0f);
+      g[j] = make_float2(1.0f, 1.0f);
+      if (nc >= p.n_out) continue;
+      const bool pair_ok = nc + 1 < p.n_out;
+      if (p.bias != nullptr) {
+        if (pair_ok) b[j] = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
+        else b[j].x = __ldg(p.bias + nc);
+      }
+      if (EPI == EPI_RESID && gate != nullptr) {
+        g[j].x = gate[nc];
+        if (pair_ok) g[j].y = gate[nc + 1];
       }
     }
-    if (EPI == EPI_QKV_ROPE) {
-      const int sec = nc / p.inner, head = (nc % p.inner) / 64;
-      if (sec < 2 && head < p.pe_heads) {
-        const int pr = (nc % 64) / 2;
-        const float c = __ldg(p.rope_cos + (long long)pos * 32 + pr), s = __ldg(p.rope_sin + (long long)pos * 32 + pr);
-        const float x0 = v0, x1 = v1;
-        v0 = x0 * c - x1 * s;
-        v1 = x1 * c + x0 * s;
+    bool rope = false;
+    float rc[2][J], rs[2][J];
+    if (EPI == EPI_QKV_ROPE) {  // inner % 64 == 0 and CW divides 64: a chunk lies in one head of one section
+      const int sec = nb / p.inner, head = (nb - sec * p.inner) >> 6;
+      rope = sec < 2 && head < p.pe_heads;
+      if (rope) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < J; ++j) {
+            const int pr = ((nb & 63) >> 1) + 4 * j + (c2 >> 1);
+            rc[h][j] = in[h] ? __ldg(p.rope_cos + (long long)pos[h] * 32 + pr) : 0.0f;
+            rs[h][j] = in[h] ? __ldg(p.rope_sin + (long long)pos[h] * 32 + pr) : 0.0f;
+          }
       }
     }
-    if (ACT == ACT_GELU_TANH) {
-      v0 = gelu_tanh(v0);
-      v1 = gelu_tanh(v1);
-    } else if (ACT == ACT_GELU_ERF) {
-      v0 = gelu_erf(v0);
-      v1 = gelu_erf(v1);
-    } else if (ACT == ACT_MISH) {
-      v0 = mish(v0);
-      v1 = mish(v1);
-    }
-    if (EPI == EPI_F16 || EPI == EPI_QKV_ROPE) {
-      __half* o = reinterpret_cast<__half*>(p.out) + grow * p.ldo + nc;
-      if (!valid) v0 = v1 = 0.0f;
-      if (pair_ok) *reinterpret_cast<uint32_t*>(o) = pack_half2(v0, v1);
-      else *o = __float2half_rn(v0);
-    } else if (EPI == EPI_F32) {
-      float* o = reinterpret_cast<float*>(p.out) + grow * p.ldo + nc;
-      if (pair_ok && !(p.ldo & 1)) {
-        *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
-      } else {
-        o[0] = v0;
-        if (pair_ok) o[1] = v1;
-      }
-      if (p.out16b != nullptr) {
-        __half* o2 = p.out16b + grow * p.ldo + nc;
-        if (!valid) v0 = v1 = 0.0f;
-        if (pair_ok && !(p.ldo & 1)) {
-          *reinterpret_cast<uint32_t*>(o2) = pack_half2(v0, v1);
-        } else {
-          o2[0] = __float2half_rn(v0);
-          if (pair_ok) o2[1] = __float2half_rn(v1);
+    float2 x[2][J];
+    if (EPI == EPI_RESID) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < J; ++j) {
+          const int nc = nb + 8 * j + c2;
+          const float* o = p.resid + grow[h] * p.ldo + nc;
+          x[h][j] = make_float2(0.0f, 0.0f);
+          if (!in[h] || nc >= p.n_out) continue;
+          if (nc + 1 < p.n_out) x[h][j] = *reinterpret_cast<const float2*>(o);  // ldo % 4 == 0, nc even: aligned
+          else x[h][j].x = o[0];
         }
-      }
-    } else if (EPI == EPI_RESID) {
-      float* o = p.resid + grow * p.ldo + nc;
-      float g0 = 1.0f, g1 = 1.0f;
-      if (gate != nullptr) {
-        g0 = gate[nc];
-        if (pair_ok) g1 = gate[nc + 1];
-      }
-      if (pair_ok) {  // ldo % 4 == 0 and nc even: 8-byte aligned
-        float2 x = *reinterpret_cast<float2*>(o);
-        x.x += g0 * v0;
-        x.y += g1 * v1;
-        *reinterpret_cast<float2*>(o) = x;
-      } else {
-        o[0] += g0 * v0;
+    }
+    // ---- math and stores ----
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!in[h]) continue;
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const int nc = nb + 8 * j + c2;
+        if (nc >= p.n_out) continue;
+        const bool pair_ok = nc + 1 < p.n_out;
+        float v0 = acc[4 * (J * cc + j) + 2 * h], v1 = acc[4 * (J * cc + j) + 2 * h + 1];
+        if (p.bias != nullptr) {
+          v0 += b[j].x;
+          if (pair_ok) v1 += b[j].y;
+        }
+        if (EPI == EPI_QKV_ROPE && rope) {
+          const float c = rc[h][j], s = rs[h][j];
+          const float x0 = v0, x1 = v1;
+          v0 = x0 * c - x1 * s;
+          v1 = x1 * c + x0 * s;
+        }
+        if (ACT == ACT_GELU_TANH) {
+          v0 = gelu_tanh(v0);
+          v1 = gelu_tanh(v1);
+        } else if (ACT == ACT_GELU_ERF) {
+          v0 = gelu_erf(v0);
+          v1 = gelu_erf(v1);
+        } else if (ACT == ACT_MISH) {
+          v0 = mish(v0);
+          v1 = mish(v1);
+        }
+        if (EPI == EPI_F16 || EPI == EPI_QKV_ROPE) {
+          __half* o = reinterpret_cast<__half*>(p.out) + grow[h] * p.ldo + nc;
+          if (!valid[h]) v0 = v1 = 0.0f;
+          if (pair_ok) *reinterpret_cast<uint32_t*>(o) = pack_half2(v0, v1);
+          else *o = __float2half_rn(v0);
+        } else if (EPI == EPI_F32) {
+          float* o = reinterpret_cast<float*>(p.out) + grow[h] * p.ldo + nc;
+          if (pair_ok && !(p.ldo & 1)) {
+            *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+          } else {
+            o[0] = v0;
+            if (pair_ok) o[1] = v1;
+          }
+          if (p.out16b != nullptr) {
+            __half* o2 = p.out16b + grow[h] * p.ldo + nc;
+            if (!valid[h]) v0 = v1 = 0.0f;
+            if (pair_ok && !(p.ldo & 1)) {
+              *reinterpret_cast<uint32_t*>(o2) = pack_half2(v0, v1);
+            } else {
+              o2[0] = __float2half_rn(v0);
+              if (pair_ok) o2[1] = __float2half_rn(v1);
+            }
+          }
+        } else if (EPI == EPI_RESID) {
+          float* o = p.resid + grow[h] * p.ldo + nc;
+          float2 xv = x[h][j];
+          if (pair_ok) {
+            xv.x += g[j].x * v0;
+            xv.y += g[j].y * v1;
+            *reinterpret_cast<float2*>(o) = xv;
+          } else {
+            o[0] = xv.x + g[j].x * v0;
+          }
+        }
       }
     }
   }
@@ -273,8 +335,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       release(prev);
-      epilogue_row<BN, EPI, ACT>(p, acc, 0, n0, c2, m0 + r_in_tile, bz, gate);
-      epilogue_row<BN, EPI, ACT>(p, acc, 1, n0, c2, m0 + r_in_tile + 8, bz, gate);
+#ifdef F5_TRACE
+      if (p.diag_no_epi) continue;  // main loop alone (F5_GEMM_EPI=none)
+#endif
+      epilogue_tile<BN, EPI, ACT>(p, acc, n0, c2, m0 + r_in_tile, bz, gate);
     }
   }
   if (PAIR) cluster_sync_all();  // the peer may still be multicasting into our smem / arriving on our barriers

@@ -36,6 +36,9 @@ struct GemmParams {
   int conv_pad;  // CONV: taps/2
   int skip_pad;    // 1: 128-row (256 for CTA pairs) tiles whose rows all lie past their sample's row_len are not computed
   int w_prefetch;  // W tiles may be loaded before griddepcontrol.wait (weights are not produced by the predecessor)
+#ifdef F5_TRACE
+  int diag_no_epi;  // instrumented build: skip the epilogue (nothing is stored) to time the main loop alone
+#endif
 };
 
 constexpr int kBM = 128;

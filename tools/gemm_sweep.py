@@ -1,4 +1,9 @@
-"""GPU tool: time the persistent wgmma GEMM per (shape, epilogue, tile) from a CUDA graph (rotating weights > L2)."""
+"""GPU tool: time the persistent wgmma GEMM per (shape, epilogue, tile) from a CUDA graph (rotating weights > L2).
+
+Every row ends with the same shape through cuBLAS (torch.matmul fp16, no epilogue) as a comparator.
+SWEEP_M=<M,...> picks the row counts; SWEEP_TILES=auto times only the planner's pick.  With the instrumented library
+(F5_LIB=f5_tts_b200/libf5tts_b200_trace.so) and F5_GEMM_EPI=none the times are of the main loop alone.
+"""
 import os
 import sys
 
@@ -29,7 +34,14 @@ def bench(M, N, K, epi, act, bn, nw=24, pair=0):
     return us, 2.0 * M * N * K / (us * 1e-6) / 1e12
 
 
+def cublas(M, N, K, nw):
+    a = [torch.randn(M, K, generator=g).half().to(DEV) for _ in range(2)]
+    wt = [(torch.randn(N, K, generator=g) / 32).half().to(DEV).t() for _ in range(nw)]
+    return _graph_time_us(lambda: [torch.matmul(a[i % 2], wt[i]) for i in range(nw)], nw, rounds=4)
+
+
 Ms = [int(x) for x in os.environ.get("SWEEP_M", "1876,3752,7504,15008").split(",")]
+pick_only = os.environ.get("SWEEP_TILES", "all") == "auto"
 for M in Ms:
     for (N, K, epi, act, tag) in ((3072, 1024, EPI_QKV_ROPE, ACT_NONE, "QKV"), (1024, 1024, EPI_RESID, ACT_NONE, "out"),
                                   (2048, 1024, EPI_F16, ACT_GELU_TANH, "FF1"), (1024, 2048, EPI_RESID, ACT_NONE, "FF2"),
@@ -38,9 +50,11 @@ for M in Ms:
             continue
         nw = -(-200_000_000 // (N * K * 2))  # distinct weights > L2 (50 MB), as in the real step
         nw = nw if M < 8000 else max(6, nw // 4)
+        auto = ops.gemm_tile(M, N, K, epi, act)
+        tiles = [(auto[0], auto[1])] if pick_only else ((128, 0), (192, 0), (256, 0), (128, 1), (192, 1), (256, 1))
         row = []
-        for bn, pair in ((128, 0), (192, 0), (256, 0), (128, 1), (192, 1), (256, 1)):
+        for bn, pair in tiles:
             us, tf = bench(M, N, K, epi, act, bn, nw=nw, pair=pair)
             row.append(f"{'P' if pair else 'bn'}{bn}: {us:6.1f}us {tf:5.0f}TF")
-        print(f"M={M:6d} {tag:7s} N={N:5d} K={K:5d} | " + " | ".join(row) + f" | auto={ops.gemm_tile(M, N, K, epi, act)}",
-              flush=True)
+        print(f"M={M:6d} {tag:7s} N={N:5d} K={K:5d} | " + " | ".join(row) + f" | auto={auto}"
+              f" | cuBLAS {cublas(M, N, K, nw):6.1f}us", flush=True)
