@@ -73,8 +73,11 @@ class SampleArgs(C.Structure):
         ("B", c_int), ("N", c_int), ("nt", c_int), ("steps", c_int),
         ("text", c_void_p), ("step_cond", c_void_p), ("y", c_void_p), ("duration", c_void_p),
         ("t", C.POINTER(c_float)), ("cfg_strength", c_float), ("trajectory", c_void_p), ("use_graph", c_int),
-        ("v_out", c_void_p), ("exact_varlen", c_int),
+        ("v_out", c_void_p), ("exact_varlen", c_int), ("method", c_int),
     ]
+
+
+ODE_METHODS = {"euler": 0, "midpoint": 1}  # SampleArgs.method; backbone evaluations per grid interval: 1 and 2
 
 
 _lock = threading.Lock()

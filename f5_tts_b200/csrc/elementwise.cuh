@@ -241,7 +241,7 @@ __global__ void grn_apply_kernel(__half* g, const float* nx, const float* gamma,
 
 // ---------------------------------------------------------------------------------------------------------
 // Input packing (backbones/dit.py:151-163): xin[Be*N, Kpad] fp16 = [ x | cond or 0 | text_emb | 0-pad ].
-// Static part once per sample(); the x columns are rewritten every step by the Euler kernel.
+// Static part once per sample(); the x columns are rewritten after every backbone evaluation by the CFG+ODE kernel.
 // ---------------------------------------------------------------------------------------------------------
 
 __global__ void pack_input_kernel(const PackParams p) {
@@ -259,9 +259,11 @@ __global__ void pack_input_kernel(const PackParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// CFG + Euler (cfm.py:190-191 + torchdiffeq fixed-grid Euler, cfm.py:218):
-//   y <- y + dt[k] * (pred + (pred - null) * cfg);  trajectory[k+1] = y;  xin[:, :mel] <- fp16(y) for both halves;
-//   the last thread-block-0 thread advances the device step counter so one captured graph serves every step.
+// CFG + one stage of torchdiffeq's fixed-grid Euler or midpoint method (cfm.py:190-191, 218), k = evaluation index:
+//   g = pred + (pred - null) * cfg;  y_stage = y + stage[k].coef * g;  xin[:, :mel] <- fp16(y_stage) for both halves;
+//   a committing stage (traj_row >= 0) also stores y <- y_stage and trajectory[traj_row] = y_stage, a midpoint half
+//   stage leaves y and the trajectory alone.  The last CTA advances the device evaluation counter, so one captured
+//   graph serves every evaluation of either method.
 // v: [Be*N, mel] fp32 (pred rows first, null rows second).
 // ---------------------------------------------------------------------------------------------------------
 
@@ -269,7 +271,7 @@ __global__ void cfg_euler_kernel(const EulerParams p) {
   pdl_wait();
   pdl_launch_dependents();
   const int k = *p.step_ptr;
-  const float dt = p.dt[k];
+  const OdeStage st = p.stage[k];
   const SampleIo io = *p.io;
   const long long total = (long long)p.BN * p.mel;
   const long long null_off = (long long)p.B * p.seq_tok * p.mel;
@@ -285,9 +287,11 @@ __global__ void cfg_euler_kernel(const EulerParams p) {
       const float nu = p.v[null_off + vi];
       g = pr + (pr - nu) * io.cfg;
     }
-    const float yn = io.y[i] + dt * g;
-    io.y[i] = yn;
-    if (io.traj) io.traj[(long long)(k + 1) * total + i] = yn;
+    const float yn = io.y[i] + st.coef * g;
+    if (st.traj_row >= 0) {
+      io.y[i] = yn;
+      if (io.traj) io.traj[(long long)st.traj_row * total + i] = yn;
+    }
     const __half h = __float2half_rn(yn);
     p.xin[r * p.Kpad + c] = h;
     if (p.packed) p.xin[(r + p.BN) * p.Kpad + c] = h;

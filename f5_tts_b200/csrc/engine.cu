@@ -1,15 +1,20 @@
 // Engine: the CFM.sample NFE loop (model/cfm.py:160-223) over a DiT (backbones/dit.py:319-370) or UNetT
 // (backbones/unett.py:244-307) backbone, expressed as a fixed kernel schedule over a caller-owned workspace.
 //
-// Per sample() call (hoisted out of the NFE loop because it is step- or batch-invariant):
+// The ODE solver is torchdiffeq's fixed-grid Euler (one backbone evaluation per grid interval, at t_k) or midpoint
+// (two: at t_k, then at t_k + dt_k/2 from the half-step state).  `evals` below counts backbone evaluations (NFE):
+// steps for Euler, 2 * steps for midpoint.
+// Per sample() call (hoisted out of the NFE loop because it is evaluation- or batch-invariant):
 //   * text embeddings, cond + uncond variants (dit.py:284-314 caches them the same way)
-//   * time embedding of every grid point and — DiT — the AdaLN modulation vectors of every (step, block)
-//     as one [steps, depth*6D + 2D] table: 22 weight-streaming GEMVs per step become one GEMM per call
+//   * time embedding of every evaluation time and — DiT — the AdaLN modulation vectors of every (evaluation, block)
+//     as one [evals, depth*6D + 2D] table: 22 weight-streaming GEMVs per evaluation become one GEMM per call
+//   * the per-evaluation solver table (OdeStage: update coefficient, trajectory row or -1)
 //   * rotary cos/sin table, static columns of the packed input projection operand
-// Per NFE step: input projection -> grouped conv position embedding x2 (tensor-core implicit GEMM) -> depth x
+// Per evaluation: input projection -> grouped conv position embedding x2 (tensor-core implicit GEMM) -> depth x
 // {norm+modulate, fused QKV+RoPE GEMM, flash attention, out-proj (+gate, +mask, +residual), norm+modulate,
-//  FF1+GELU, FF2 (+gate, +residual)} -> final norm -> proj_out -> fused CFG + Euler update.
-// Every kernel reads the step index from a device counter, so one captured CUDA graph serves all steps.
+//  FF1+GELU, FF2 (+gate, +residual)} -> final norm -> proj_out -> fused CFG + ODE stage update.
+// Every kernel reads the evaluation index from a device counter, so one captured CUDA graph serves all evaluations
+// of either method: the method reaches the graph only through the tables the prologue writes.
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -37,13 +42,13 @@ struct Bump {
 
 struct Layout {
   // sizes
-  int B, Be, N, seq, steps, packed;
+  int B, Be, N, seq, evals, packed;  // evals: backbone evaluations per call (steps, or 2 * steps for midpoint)
   long long M, M1;
   // common
-  int* step_ptr;
+  int* step_ptr;    // [0]: evaluation counter
   SampleIo* io;     // caller tensors + cfg scale of THIS call, read by the step kernels through the workspace
-  float* dt;
-  float* t_dev;
+  OdeStage* stage;  // [evals]
+  float* t_dev;     // [evals] evaluation times
   float *rope_cos, *rope_sin;
   int* row_len;     // [Be] or unused
   int* kv_len;      // [Be] or unused
@@ -76,8 +81,11 @@ using namespace f5;
 // One instantiated step graph.  The graph touches only the workspace: the caller's tensors (y, trajectory) and the CFG
 // scale reach the kernels through the SampleIo block the prologue writes into the workspace, so the cache key is the
 // workspace address plus the shape parameters the layout / kernel plans depend on — a fresh `y` or `trajectory`
-// allocation per call no longer forces a re-capture.  Entries are reference-counted: a launch in flight on one thread
-// keeps its graph alive while another thread evicts it.
+// allocation per call no longer forces a re-capture.  The ODE method is not in the key: it only changes the contents
+// of the time, modulation and OdeStage tables, which every call's prologue rewrites, while `evals` fixes where those
+// tables sit in the workspace.  So Euler over 2S steps and midpoint over S steps replay the same graph, each with its
+// own tables, and an Euler and a midpoint call with different `evals` never share one.  Entries are reference-counted:
+// a launch in flight on one thread keeps its graph alive while another thread evicts it.
 struct GraphHolder {
   cudaGraphExec_t exec = nullptr;
   int nodes = 0;  // kernel/memcpy nodes per replay (for the launch counter)
@@ -87,9 +95,9 @@ struct GraphHolder {
 };
 struct GraphKey {
   const void* ws;
-  int B, N, steps, packed, masked;  // masked: 0 = no lengths, 1 = lengths (reference batched semantics), 2 = exact_varlen
+  int B, N, evals, packed, masked;  // masked: 0 = no lengths, 1 = lengths (reference batched semantics), 2 = exact_varlen
   bool operator==(const GraphKey& o) const {
-    return ws == o.ws && B == o.B && N == o.N && steps == o.steps && packed == o.packed && masked == o.masked;
+    return ws == o.ws && B == o.B && N == o.N && evals == o.evals && packed == o.packed && masked == o.masked;
   }
 };
 struct GraphEntry {
@@ -106,12 +114,12 @@ struct f5_engine {
   std::vector<GraphEntry> graphs;
 };
 
-static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int steps, float cfg) {
+static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int evals, float cfg) {
   const f5_arch& A = e->arch;
   Bump bp(ws);
   L.B = B;
   L.N = N;
-  L.steps = steps;
+  L.evals = evals;
   L.packed = cfg < 1e-5f ? 0 : 1;
   L.Be = L.packed ? 2 * B : B;
   L.seq = A.backbone == 1 ? N + 1 : N;
@@ -120,19 +128,19 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   const int D = A.dim, Td = A.text_dim, F = A.ff_inner;
   L.step_ptr = bp.take<int>(64);
   L.io = bp.take<SampleIo>(1);
-  L.dt = bp.take<float>(steps + 1);
-  L.t_dev = bp.take<float>(steps + 1);
+  L.stage = bp.take<OdeStage>(evals);
+  L.t_dev = bp.take<float>(evals);
   L.rope_cos = bp.take<float>((size_t)L.seq * 32);
   L.rope_sin = bp.take<float>((size_t)L.seq * 32);
   L.row_len = bp.take<int>(L.Be);
   L.kv_len = bp.take<int>(L.Be);
   L.frame_len = bp.take<int>(L.Be);
   L.valid_len = bp.take<int>(B);
-  L.tfeat = bp.take<float>((size_t)steps * 256);
-  L.th1 = bp.take<float>((size_t)steps * D);
-  L.temb = bp.take<float>((size_t)steps * D);
-  L.temb_silu = bp.take<__half>((size_t)steps * D);
-  L.mod = bp.take<float>((size_t)steps * (e->modW > 0 ? e->modW : 1));
+  L.tfeat = bp.take<float>((size_t)evals * 256);
+  L.th1 = bp.take<float>((size_t)evals * D);
+  L.temb = bp.take<float>((size_t)evals * D);
+  L.temb_silu = bp.take<__half>((size_t)evals * D);
+  L.mod = bp.take<float>((size_t)evals * (e->modW > 0 ? e->modW : 1));
   L.tx = bp.take<float>((size_t)2 * B * N * Td);
   L.filler = bp.take<uint8_t>((size_t)B * N);
   L.ta = bp.take<__half>((size_t)2 * B * N * Td);
@@ -207,13 +215,13 @@ void f5_engine_destroy(f5_engine* e) {
   delete e;  // graph holders destroy their executables
 }
 
-size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int steps, float cfg_strength) {
+size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
   Layout L;
-  plan_layout(e, L, nullptr, B, N, steps, cfg_strength);
+  plan_layout(e, L, nullptr, B, N, nfe, cfg_strength);
   return L.bytes;
 }
 
-double f5_sample_flops(const f5_engine* e, int B, int N, int steps, float cfg_strength) {
+double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
   const f5_arch& A = e->arch;
   const double D = A.dim, mel = A.mel_dim, Td = A.text_dim, F = A.ff_inner, Ld = A.depth;
   const double Be = cfg_strength < 1e-5f ? B : 2.0 * B;
@@ -227,11 +235,11 @@ double f5_sample_flops(const f5_engine* e, int B, int N, int steps, float cfg_st
     per = Ld * (8.0 * n1 * D * D + 4.0 * n1 * D * F + 4.0 * n1 * n1 * D) + (Ld / 2.0) * 4.0 * n1 * D * D +
           2.0 * n * (2 * mel + Td) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n1 * D * mel;
   }
-  double total = steps * Be * per;
+  double total = nfe * Be * per;
   // text embedding, once per sample and CFG branch: conv_layers x (2 pointwise GEMMs)
   total += 2.0 * B * A.conv_layers * (2.0 * 2.0 * N * Td * 2.0 * Td);
-  // conditioning: time MLP + AdaLN table, once per call
-  total += steps * (2.0 * 256 * D + 2.0 * D * D + 2.0 * D * (double)e->modW);
+  // conditioning: time MLP + AdaLN table, one row per evaluation, computed once per call
+  total += nfe * (2.0 * 256 * D + 2.0 * D * D + 2.0 * D * (double)e->modW);
   return total;
 }
 
@@ -479,7 +487,7 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
   ep.io = L.io;
   ep.v = L.v;
   ep.xin = L.xin;
-  ep.dt = L.dt;
+  ep.stage = L.stage;
   ep.step_ptr = L.step_ptr;
   ep.BN = L.B * L.N;
   ep.mel = A.mel_dim;
@@ -495,15 +503,33 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
 int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaStream_t s) {
   const f5_arch& A = e->arch;
   const f5_weights& W = e->w;
-  const int D = A.dim, Td = A.text_dim, B = L.B, N = L.N, S = L.steps;
+  const int D = A.dim, Td = A.text_dim, B = L.B, N = L.N, S = L.evals;
   const bool dit = A.backbone == 0;
   const bool masked = sa->duration != nullptr;
   const bool strict = masked && sa->exact_varlen;
-  // small host -> device control data (pageable source: cudaMemcpyAsync stages it before returning)
-  std::vector<float> dt(S + 1, 0.f);
-  for (int k = 0; k < S; ++k) dt[k] = sa->t[k + 1] - sa->t[k];
-  RC(check_cuda(cudaMemcpyAsync(L.dt, dt.data(), sizeof(float) * (S + 1), cudaMemcpyHostToDevice, s), "dt h2d"));
-  RC(check_cuda(cudaMemcpyAsync(L.t_dev, sa->t, sizeof(float) * (S + 1), cudaMemcpyHostToDevice, s), "t h2d"));
+  // small host -> device control data (pageable source: cudaMemcpyAsync stages it before returning).
+  // Per grid interval k (torchdiffeq's fixed-grid solvers): Euler evaluates at t_k and commits y + dt_k * g; midpoint
+  // evaluates at t_k, forms y + half_dt_k * g as the next evaluation's input only, then evaluates at t_k + half_dt_k
+  // and commits y + dt_k * g.  Times are fp32 (the reference builds the grid in the parameter dtype).
+  std::vector<OdeStage> stage;
+  std::vector<float> te;
+  stage.reserve(S);
+  te.reserve(S);
+  for (int k = 0; k < sa->steps; ++k) {
+    const float dt = sa->t[k + 1] - sa->t[k];
+    if (sa->method == 1) {
+      const float half_dt = 0.5f * dt;
+      te.push_back(sa->t[k]);
+      stage.push_back(OdeStage{half_dt, -1});
+      te.push_back(sa->t[k] + half_dt);
+      stage.push_back(OdeStage{dt, k + 1});
+    } else {
+      te.push_back(sa->t[k]);
+      stage.push_back(OdeStage{dt, k + 1});
+    }
+  }
+  RC(check_cuda(cudaMemcpyAsync(L.stage, stage.data(), sizeof(OdeStage) * S, cudaMemcpyHostToDevice, s), "stage h2d"));
+  RC(check_cuda(cudaMemcpyAsync(L.t_dev, te.data(), sizeof(float) * S, cudaMemcpyHostToDevice, s), "t h2d"));
   RC(check_cuda(cudaMemsetAsync(L.step_ptr, 0, sizeof(int) * 64, s), "step memset"));
   SampleIo io{sa->y, sa->trajectory, sa->cfg_strength};
   RC(check_cuda(cudaMemcpyAsync(L.io, &io, sizeof(io), cudaMemcpyHostToDevice, s), "io h2d"));
@@ -530,7 +556,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     }
   }
   RC(run_rope_table(L.rope_cos, L.rope_sin, L.seq, 32, s));
-  // time embedding for every grid point (modules.py:852-862)
+  // time embedding for every evaluation time (modules.py:852-862)
   RC(run_time_features(L.t_dev, L.tfeat, S, 256, s));
   RC(run_small_linear(1, L.tfeat, reinterpret_cast<const __half*>(W.time_w0), W.time_b0, L.th1, S, 256, D, s));
   RC(run_small_linear(0, L.th1, reinterpret_cast<const __half*>(W.time_w1), W.time_b1, L.temb, S, D, D, s));
@@ -631,15 +657,20 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
     set_error("f5_sample: empty problem (B=%d N=%d steps=%d nt=%d)", sa->B, sa->N, sa->steps, sa->nt);
     return -1;
   }
+  if (sa->method != 0 && sa->method != 1) {
+    set_error("f5_sample: method must be 0 (euler) or 1 (midpoint), got %d", sa->method);
+    return -1;
+  }
+  const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
   Layout L;
-  plan_layout(e, L, workspace, sa->B, sa->N, sa->steps, sa->cfg_strength);
+  plan_layout(e, L, workspace, sa->B, sa->N, evals, sa->cfg_strength);
   if (ws_bytes < L.bytes) {
     set_error("f5_sample: workspace too small (%zu < %zu)", ws_bytes, L.bytes);
     return -1;
   }
   RC(run_prologue(e, L, sa, s));
   if (sa->use_graph) {
-    const GraphKey key{workspace, sa->B, sa->N, sa->steps, L.packed,
+    const GraphKey key{workspace, sa->B, sa->N, evals, L.packed,
                        sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1)};
     std::shared_ptr<GraphHolder> g;
     {
@@ -682,12 +713,12 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
       if (e->graphs.size() >= 16) e->graphs.erase(e->graphs.begin());  // holder is freed when its last user is done
       e->graphs.push_back(GraphEntry{key, g});
     }
-    for (int k = 0; k < sa->steps; ++k) RC(check_cuda(cudaGraphLaunch(g->exec, s), "graph launch"));
-    count_launch(g->nodes * sa->steps);
+    for (int k = 0; k < evals; ++k) RC(check_cuda(cudaGraphLaunch(g->exec, s), "graph launch"));
+    count_launch(g->nodes * evals);
     return copy_v_out(e, L, sa, s);
   }
   StepPlans P;
   RC(build_step_plans(e, L, sa, P));
-  for (int k = 0; k < sa->steps; ++k) RC(run_step(e, L, sa, P, s));
+  for (int k = 0; k < evals; ++k) RC(run_step(e, L, sa, P, s));
   return copy_v_out(e, L, sa, s);
 }

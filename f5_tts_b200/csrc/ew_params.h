@@ -56,11 +56,19 @@ struct SampleIo {
   float cfg;    // classifier-free-guidance scale
 };
 
+// One backbone evaluation of the fixed-grid ODE solver: y_stage = y + coef * g.  traj_row >= 0 commits the stage
+// (y <- y_stage, trajectory[traj_row] = y_stage); traj_row < 0 is a midpoint half stage, which only reaches the next
+// evaluation through the fp16 x columns of xin.  Euler: (dt_k, k+1).  Midpoint: (dt_k / 2, -1), then (dt_k, k+1).
+struct OdeStage {
+  float coef;
+  int traj_row;
+};
+
 struct EulerParams {
   const SampleIo* io;
   const float* v;  // [Be*N, mel]
   __half* xin;
-  const float* dt;  // [steps] device
+  const OdeStage* stage;  // [evals] device, indexed by the evaluation counter
   int* step_ptr;
   int BN, mel, Kpad, packed;
   int N;         // frames per sample

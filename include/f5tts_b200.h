@@ -163,9 +163,9 @@ typedef struct {
   const int* duration;       /* device int32 [B] per-sample lengths = `mask` of cfm.py:155-158, or NULL (B == 1) */
   const float* t;            /* HOST fp32 [steps+1] time grid after EPSS / sway (cfm.py:211-216) */
   float cfg_strength;        /* < 1e-5 -> single un-packed forward (cfm.py:166-177) */
-  float* trajectory;         /* device fp32 [steps+1, B, N, mel] or NULL */
-  int use_graph;             /* capture one NFE step into a CUDA graph and replay it */
-  float* v_out;              /* optional device fp32 [Be, N, mel]: raw backbone output of the LAST step (the value
+  float* trajectory;         /* device fp32 [steps+1, B, N, mel] or NULL: y at the grid points only, for either method */
+  int use_graph;             /* capture one backbone evaluation into a CUDA graph and replay it once per evaluation */
+  float* v_out;              /* optional device fp32 [Be, N, mel]: raw backbone output of the LAST evaluation (the value
                                 transformer(x, cond, text, time, mask, cfg_infer=...) returns, dit.py:367-370) */
   int exact_varlen;          /* with duration != NULL: 1 = every sample is computed exactly as if it were ALONE in the batch
                                 with N = duration[b] — text blocks, conv position embedding and attention see nothing past
@@ -173,12 +173,17 @@ typedef struct {
                                 computes (the reference's per-chunk loop, infer/utils_infer.py:540-541), in one batch.
                                 0 = the reference's batched semantics (padded rows computed; attended unless
                                 arch.attn_mask_enabled) */
+  int method;                /* 0 = euler, 1 = midpoint: torchdiffeq's fixed-grid method (odeint_kwargs, cfm.py:39-43,
+                                218).  Euler makes `steps` backbone evaluations, midpoint 2 * steps (at t_k and at
+                                t_k + dt_k/2).  Any other value is rejected. */
 } f5_sample_args;
-size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int steps, float cfg_strength);
+/* nfe: backbone evaluations of the call — steps for euler, 2 * steps for midpoint */
+size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, float cfg_strength);
 int f5_sample(f5_engine* e, const f5_sample_args* args, void* workspace, size_t ws_bytes, f5_stream_t stream);
 
-/* algorithmic FLOPs of one f5_sample call (SURVEY.md §8d formula) — used by bench.py for the roofline */
-double f5_sample_flops(const f5_engine* e, int B, int N, int steps, float cfg_strength);
+/* algorithmic FLOPs of one f5_sample call making nfe backbone evaluations (SURVEY.md §8d formula) — used by bench.py
+ * for the roofline */
+double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength);
 
 #ifdef __cplusplus
 }
