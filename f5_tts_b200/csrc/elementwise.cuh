@@ -308,12 +308,6 @@ __global__ void cfg_euler_kernel(const EulerParams p) {
   }
 }
 
-__global__ void advance_step_kernel(int* step_ptr) {
-  pdl_wait();
-  pdl_launch_dependents();
-  *step_ptr += 1;
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // Small fp32 linear for the per-sample() conditioning MLPs (modules.py:852-862): out[s, n] = act(in[s,:] . W[n,:] + b)
 // W fp16 [Nout, K]; one warp per output column, S <= 64 rows.
@@ -373,11 +367,6 @@ __global__ void time_features_kernel(const float* t, float* feat, int S, int dim
 __global__ void silu_to_half_kernel(const float* in, __half* out, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     out[i] = __float2half_rn(silu(in[i]));
-}
-
-__global__ void float_to_half_kernel(const float* in, __half* out, long long n) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    out[i] = __float2half_rn(in[i]);
 }
 
 // rotary tables (x_transformers RotaryEmbedding, dit.py:207,352): cos/sin[pos, i] of pos * 10000^(-2i/dh)

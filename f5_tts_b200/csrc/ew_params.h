@@ -1,7 +1,8 @@
-// Parameter blocks of the bandwidth-bound kernels (plain structs shared between ops.cu and engine.cu).
+// Parameter blocks of the bandwidth-bound kernels (plain structs shared between ops.cu, engine.cu and kernel_hooks.cu).
 #pragma once
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include <vector_types.h>
 
 namespace f5 {
 
@@ -75,6 +76,14 @@ struct EulerParams {
   int seq_tok;   // rows per sample in v (N for DiT, N + 1 for UNetT)
   int tok_off;   // first frame row inside a sample of v (0 DiT, 1 UNetT: skips the time token, unett.py:305)
   int B;
+};
+
+// Constant tables of the FFT kernels, built once per device by fft_tables_kernel (ops.cu: fft_tables()):
+//   tw[k]   = (cos, sin)(2 pi k / 1024), k = 0..511   (w_1024^k; w_512^j = w_1024^{2j})
+//   hann[i] = 0.5 - 0.5 cos(2 pi i / 1024)            (periodic Hann, torch.hann_window(1024))
+struct FftTables {
+  const float2* tw;
+  const float* hann;
 };
 
 }  // namespace f5

@@ -5,6 +5,7 @@
 // lives in shared memory (8 KB data + 4 KB twiddles); global traffic is the algorithmic minimum.
 #pragma once
 #include "common.cuh"
+#include "ew_params.h"
 
 namespace f5 {
 
@@ -39,14 +40,7 @@ __device__ __forceinline__ void fft1024_inplace(float* re, float* im, const floa
   }
 }
 
-// Constant tables, built once per device by fft_tables_kernel (ops.cu: fft_tables()):
-//   tw[k]   = (cos, sin)(2 pi k / 1024), k = 0..511   (w_1024^k; w_512^j = w_1024^{2j})
-//   hann[i] = 0.5 - 0.5 cos(2 pi i / 1024)            (periodic Hann, torch.hann_window(1024))
-struct FftTables {
-  const float2* tw;
-  const float* hann;
-};
-
+// FftTables (twiddles, Hann window): ew_params.h
 __global__ void fft_tables_kernel(float2* tw, float* hann) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < kNfft / 2) {
@@ -76,12 +70,13 @@ __device__ __forceinline__ int bitrev9(int i) { return int(__brev(unsigned(i)) >
 // complex radix-2 FFT (9 stages, one butterfly per thread and stage) is followed by the split
 //   X[k] = (Z[k] + conj Z[512-k]) / 2  -  i w_1024^k (Z[k] - conj Z[512-k]) / 2,   k = 0..512,
 // i.e. half the butterflies of a 1024-point complex transform.  Twiddles and window come from per-device tables.
-// Filterbank: fb is the dense [513, n_mels] matrix of the reference (triangular HTK filters: ~2 % non-zero); filter m
-// is non-zero only on bins [lo[m], hi[m]], so thread m sums that range only (host-built index, ops.cu).
+// Filterbank: fb is the caller's dense [513, n_mels] matrix, read as it is at launch time (no host-side index keyed
+// by its address, so a rewritten or reallocated filterbank is always seen as it is).  Thread m sums all 513 bins in
+// ascending order; fb loads are coalesced across m.  The zero entries of a triangular filter add exact zeros, so the
+// result equals a sum over the filter's non-zero band only.
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) mel_stft_kernel(const float* wav, int nw, int T, const float* fb, int n_mels,
-                                                        const short* band_lo, const short* band_hi, FftTables tab,
-                                                        float* out, int out_btc) {
+                                                        FftTables tab, float* out, int out_btc) {
   __shared__ float re[kNfft / 2 + 1], im[kNfft / 2 + 1], twc[kNfft / 2], tws[kNfft / 2], mag[kBins];
   const int t = blockIdx.x, b = blockIdx.y;
   load_twiddles(twc, tws, tab.tw);
@@ -137,8 +132,7 @@ __global__ void __launch_bounds__(256) mel_stft_kernel(const float* wav, int nw,
   __syncthreads();
   for (int m = threadIdx.x; m < n_mels; m += 256) {
     float acc = 0.f;
-    const int lo = band_lo[m], hi = band_hi[m];
-    for (int f = lo; f <= hi; ++f) acc += mag[f] * __ldg(fb + f * n_mels + m);
+    for (int f = 0; f < kBins; ++f) acc += mag[f] * __ldg(fb + f * n_mels + m);
     const float v = logf(fmaxf(acc, 1e-5f));
     if (out_btc) out[((long long)b * T + t) * n_mels + m] = v;
     else out[((long long)b * n_mels + m) * T + t] = v;

@@ -94,4 +94,12 @@ int run_rope_table(float* cs, float* sn, int seq, int half, cudaStream_t s);
 int run_prepend_time_token(float* dst, const float* src, const float* t_emb, const int* step_ptr, int N, int D,
                            long long rows_out, cudaStream_t s);
 int run_concat_half(const float* x, const float* skip, __half* out, long long rows, int D, cudaStream_t s);
+
+// ---- FFT tables and the Vocos kernels outside the GEMMs (ops.cu) ----
+int fft_tables(FftTables* out, cudaStream_t s);  // built once per device; complete when this returns
+int run_vocos_im2col(const float* mel, int B, int C, int T, __half* A, int Kpad, cudaStream_t s);
+int run_ln_affine_f32(const float* x, float* out, int rows, int D, float eps, const float* w, const float* b,
+                      cudaStream_t s);
+// head [B*T, ld] (log-magnitude | phase) -> frames [B*T, 1024] scratch -> wav [B, 256 (T-1)]
+int run_istft(const float* head, int ld, float* frames, float* wav, int B, int T, FftTables tab, cudaStream_t s);
 }  // namespace f5

@@ -12,14 +12,13 @@
 
 namespace f5 {
 
-// ---- per-device constant tables of the FFT kernels (twiddles, Hann window) and per-filterbank band indices ----------
+// ---- per-device constant tables of the FFT kernels (twiddles, Hann window) ----------------------------------------
 namespace {
 std::mutex g_fft_mu;
-std::map<int, FftTables> g_fft_tables;                                  // device ordinal -> tables
-std::map<std::pair<int, const void*>, std::pair<short*, short*>> g_bands;  // (device, fb pointer) -> (lo, hi) [n_mels]
+std::map<int, FftTables> g_fft_tables;  // device ordinal -> tables
 }  // namespace
 
-static int fft_tables(FftTables* out, cudaStream_t s) {
+int fft_tables(FftTables* out, cudaStream_t s) {
   int dev = 0;
   cudaGetDevice(&dev);
   std::lock_guard<std::mutex> lk(g_fft_mu);
@@ -36,48 +35,6 @@ static int fft_tables(FftTables* out, cudaStream_t s) {
     it = g_fft_tables.emplace(dev, FftTables{tw, hann}).first;
   }
   *out = it->second;
-  return 0;
-}
-
-// First / last non-zero bin of every mel filter of the caller's dense [513, n_mels] filterbank (one D2H read per
-// filterbank tensor; the Python side keeps one per device).
-static int mel_bands(const float* fb, int n_mels, const short** lo, const short** hi, cudaStream_t s) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lk(g_fft_mu);
-  const auto key = std::make_pair(dev, static_cast<const void*>(fb));
-  auto it = g_bands.find(key);
-  if (it == g_bands.end()) {
-    std::vector<float> h((size_t)kBins * n_mels);
-    if (int rc = check_cuda(cudaMemcpyAsync(h.data(), fb, sizeof(float) * h.size(), cudaMemcpyDeviceToHost, s), "fb d2h")) return rc;
-    if (int rc = check_cuda(cudaStreamSynchronize(s), "fb sync")) return rc;
-    std::vector<short> l(n_mels, 1), u(n_mels, 0);  // empty band: lo > hi
-    for (int m = 0; m < n_mels; ++m) {
-      int first = -1, last = -1;
-      for (int f = 0; f < kBins; ++f)
-        if (h[(size_t)f * n_mels + m] != 0.0f) {
-          if (first < 0) first = f;
-          last = f;
-        }
-      if (first >= 0) l[m] = (short)first, u[m] = (short)last;
-    }
-    short *dl = nullptr, *du = nullptr;
-    if (int rc = check_cuda(cudaMalloc(&dl, sizeof(short) * n_mels), "band index")) return rc;
-    if (int rc = check_cuda(cudaMalloc(&du, sizeof(short) * n_mels), "band index")) return rc;
-    cudaMemcpyAsync(dl, l.data(), sizeof(short) * n_mels, cudaMemcpyHostToDevice, s);
-    cudaMemcpyAsync(du, u.data(), sizeof(short) * n_mels, cudaMemcpyHostToDevice, s);
-    if (int rc = check_cuda(cudaStreamSynchronize(s), "band index sync")) return rc;
-    if (g_bands.size() >= 64) {  // filterbanks are per-process constants; a churning caller must not leak without bound
-      for (auto& kv : g_bands) {
-        cudaFree(kv.second.first);
-        cudaFree(kv.second.second);
-      }
-      g_bands.clear();
-    }
-    it = g_bands.emplace(key, std::make_pair(dl, du)).first;
-  }
-  *lo = it->second.first;
-  *hi = it->second.second;
   return 0;
 }
 
@@ -214,6 +171,27 @@ int run_concat_half(const float* x, const float* skip, __half* out, long long ro
   return check_launch("concat_half_kernel");
 }
 
+int run_vocos_im2col(const float* mel, int B, int C, int T, __half* A, int Kpad, cudaStream_t s) {
+  vocos_im2col_kernel<<<B * T, 256, 0, s>>>(mel, B, C, T, A, Kpad);
+  count_launch();
+  return check_launch("vocos_im2col_kernel");
+}
+
+int run_ln_affine_f32(const float* x, float* out, int rows, int D, float eps, const float* w, const float* b,
+                      cudaStream_t s) {
+  ln_affine_f32_kernel<<<(rows + 7) / 8, 256, 0, s>>>(x, out, rows, D, eps, w, b);
+  count_launch();
+  return check_launch("ln_affine_f32_kernel");
+}
+
+int run_istft(const float* head, int ld, float* frames, float* wav, int B, int T, FftTables tab, cudaStream_t s) {
+  istft_frames_kernel<<<B * T, 256, 0, s>>>(head, ld, frames, tab);
+  const long long total = (long long)B * kHop * (T - 1);
+  istft_ola_kernel<<<grid_for(total, 256), 256, 0, s>>>(frames, T, wav, B, tab);
+  count_launch(2);
+  return check_launch("vocos istft kernels");
+}
+
 }  // namespace f5
 
 using namespace f5;
@@ -243,9 +221,7 @@ int f5_mel_spectrogram(const float* wav, int B, int nw, const float* fb, int n_m
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   FftTables tab;
   if (int rc = fft_tables(&tab, s)) return rc;
-  const short *lo = nullptr, *hi = nullptr;
-  if (int rc = mel_bands(fb, n_mels, &lo, &hi, s)) return rc;
-  mel_stft_kernel<<<dim3(T, B), 256, 0, s>>>(wav, nw, T, fb, n_mels, lo, hi, tab, out, out_btc);
+  mel_stft_kernel<<<dim3(T, B), 256, 0, s>>>(wav, nw, T, fb, n_mels, tab, out, out_btc);
   count_launch();
   return check_launch("mel_stft_kernel");
 }
@@ -289,17 +265,14 @@ int vocos_enqueue(const f5_vocos_weights* w, const float* mel, int B, int T, voi
   float* frames = reinterpret_cast<float*>(take((size_t)R * 1024 * 4));
 
   int rc;
-  vocos_im2col_kernel<<<R, 256, 0, s>>>(mel, B, 100, T, A0, 704);
-  count_launch();
+  if ((rc = run_vocos_im2col(mel, B, 100, T, A0, 704, s))) return rc;
   f5_gemm_args ga{};
   ga.weights_static = 1;
   ga.rows = R; ga.batches = 1; ga.n_out = 512; ga.k = 704; ga.lda = 704; ga.ldw = 704; ga.bn = 64;
   ga.epi = F5_EPI_F32; ga.act = F5_ACT_NONE; ga.bias = w->embed_b; ga.out = e; ga.ldo = 512;
   if ((rc = f5_gemm(A0, w->embed_w, &ga, stream))) return rc;
   // x = LayerNorm(embed(mel)) is the residual stream (fp32)
-  ln_affine_f32_kernel<<<(R + 7) / 8, 256, 0, s>>>(e, x, R, 512, 1e-6f, w->norm_w, w->norm_b);
-  count_launch();
-  if ((rc = check_launch("ln_affine_f32_kernel"))) return rc;
+  if ((rc = run_ln_affine_f32(e, x, R, 512, 1e-6f, w->norm_w, w->norm_b, s))) return rc;
   for (int i = 0; i < w->layers; ++i) {
     DwConvLnParams dp{};
     dp.x = x; dp.out = a; dp.B = B; dp.N = T; dp.C = 512; dp.w = w->dw_w[i]; dp.wb = w->dw_b[i];
@@ -327,11 +300,7 @@ int vocos_enqueue(const f5_vocos_weights* w, const float* mel, int B, int T, voi
   gh.rows = R; gh.batches = 1; gh.n_out = 1026; gh.k = 512; gh.lda = 512; gh.ldw = 512; gh.bn = 128;
   gh.epi = F5_EPI_F32; gh.act = F5_ACT_NONE; gh.bias = w->head_b; gh.out = head; gh.ldo = 1026;
   if ((rc = f5_gemm(a, w->head_w, &gh, stream))) return rc;
-  istft_frames_kernel<<<R, 256, 0, s>>>(head, 1026, frames, tab);
-  const long long total = (long long)B * kHop * (T - 1);
-  istft_ola_kernel<<<grid_for(total, 256), 256, 0, s>>>(frames, T, wav, B, tab);
-  count_launch(2);
-  return check_launch("vocos istft kernels");
+  return run_istft(head, 1026, frames, wav, B, T, tab, s);
 }
 
 // One captured decode per (weights, workspace, B, T).  Only two kernels touch caller tensors — the im2col reads `mel`, the
