@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_90a kernels: mbarrier, TMA, cluster and wgmma-descriptor wrappers (inline PTX),
-// small math.  No torch, no CUTLASS — plain CUDA 12.9.
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA load, programmatic-dependent-launch and
+// wgmma-descriptor wrappers (inline PTX), small math.  No torch, no CUTLASS — plain CUDA 12.9.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -57,21 +57,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// non-blocking phase test (acquire): lets one thread multiplex several producer/consumer streams
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-
-// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-
 // ----------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor), tile mode, mbarrier completion
 // ----------------------------------------------------------------------------------------------
@@ -91,59 +76,6 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
           "r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-
-// bulk tensor stores smem -> global (the issuing thread owns the bulk async-group)
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-// global[tile] += smem[tile]  (element type from the tensor map: fp32)
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
-  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// the same box lands at the same shared-memory offset in every CTA of `cta_mask`, and its bytes are credited to the
-// mbarrier at the same offset in each of them
-__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                                      uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
-      "%4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
-      : "memory");
-}
-
-// ---- clusters ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the offset of `bar` inside CTA `rank` of the cluster (the own CTA included)
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)),
-      "r"(rank)
       : "memory");
 }
 

@@ -48,11 +48,6 @@ static EncodeTiledFn get_encode_fn() {
 
 int encode_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                     uint64_t stride2, uint32_t b0, uint32_t b1, int rank) {
-  return encode_tmap(m, 0, ptr, d0, d1, d2, stride1, stride2, b0, b1, rank);
-}
-
-int encode_tmap(CUtensorMap* m, int is_f32, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
-                uint64_t stride2, uint32_t b0, uint32_t b1, int rank) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver / not a TMA-capable device)");
@@ -67,7 +62,7 @@ int encode_tmap(CUtensorMap* m, int is_f32, const void* ptr, uint64_t d0, uint64
   cuuint64_t strides[2] = {stride1, stride2};
   cuuint32_t box[3] = {b0, b1, 1};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(m, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -78,37 +73,47 @@ int encode_tmap(CUtensorMap* m, int is_f32, const void* ptr, uint64_t d0, uint64
   return 0;
 }
 
-int configure_kernels();
-int num_sms();
+// Every instantiated GEMM kernel.  configure_kernels sets them all up, gemm_run launches the entry that matches a plan,
+// and pick_tile only considers widths that have an entry for the epilogue.
+struct GemmKernel {
+  int bn, epi, act;
+  bool conv;
+  void (*fn)(CUtensorMap, CUtensorMap, GemmParams);
+};
+#define F5_GEMM_KERNEL(BN, EPI, ACT, CONV) {BN, EPI, ACT, CONV, gemm_wgmma_kernel<BN, EPI, ACT, CONV>}
+static const GemmKernel kGemmKernels[] = {
+    F5_GEMM_KERNEL(64, EPI_F16, ACT_NONE, false),
+    F5_GEMM_KERNEL(64, EPI_F16, ACT_GELU_TANH, false),
+    F5_GEMM_KERNEL(64, EPI_F16, ACT_GELU_ERF, false),
+    F5_GEMM_KERNEL(64, EPI_F32, ACT_NONE, false),
+    F5_GEMM_KERNEL(64, EPI_RESID, ACT_NONE, false),
+    F5_GEMM_KERNEL(128, EPI_F16, ACT_NONE, false),
+    F5_GEMM_KERNEL(128, EPI_F16, ACT_GELU_TANH, false),
+    F5_GEMM_KERNEL(128, EPI_F16, ACT_GELU_ERF, false),
+    F5_GEMM_KERNEL(128, EPI_F32, ACT_NONE, false),
+    F5_GEMM_KERNEL(128, EPI_RESID, ACT_NONE, false),
+    F5_GEMM_KERNEL(256, EPI_F16, ACT_NONE, false),
+    F5_GEMM_KERNEL(256, EPI_F16, ACT_GELU_TANH, false),
+    F5_GEMM_KERNEL(256, EPI_F16, ACT_GELU_ERF, false),
+    F5_GEMM_KERNEL(256, EPI_F32, ACT_NONE, false),
+    F5_GEMM_KERNEL(256, EPI_RESID, ACT_NONE, false),
+    F5_GEMM_KERNEL(128, EPI_QKV_ROPE, ACT_NONE, false),
+    F5_GEMM_KERNEL(192, EPI_QKV_ROPE, ACT_NONE, false),
+    F5_GEMM_KERNEL(192, EPI_F16, ACT_NONE, false),
+    F5_GEMM_KERNEL(192, EPI_F16, ACT_GELU_TANH, false),
+    F5_GEMM_KERNEL(192, EPI_RESID, ACT_NONE, false),
+    F5_GEMM_KERNEL(256, EPI_QKV_ROPE, ACT_NONE, false),
+    F5_GEMM_KERNEL(64, EPI_F16, ACT_MISH, true),
+    F5_GEMM_KERNEL(64, EPI_RESID, ACT_MISH, true),
+};
+#undef F5_GEMM_KERNEL
 
-template <int BN, int STAGES, int EPI, int ACT, bool CONV, bool PAIR = false>
-static int launch_inst(const GemmPlan& pl, cudaStream_t s) {
-  auto kern = gemm_wgmma_kernel<BN, STAGES, EPI, ACT, CONV, PAIR>;
-  constexpr size_t smem = gemm_smem_bytes<BN, STAGES>();
-  if (int rc = configure_kernels()) return rc;
-  PdlLaunch L(pl.grid, dim3(kGemmThreads), smem, s, PAIR ? 2 : 1);
-  if (int rc = check_cuda(cudaLaunchKernelEx(&L.cfg, kern, pl.tmA, pl.tmB, pl.p), "gemm launch")) return rc;
-  count_launch();
-  return check_launch("gemm_wgmma_kernel launch");
+static const GemmKernel* find_kernel(int bn, int epi, int act, bool conv) {
+  for (const GemmKernel& k : kGemmKernels)
+    if (k.bn == bn && k.epi == epi && k.act == act && k.conv == conv) return &k;
+  return nullptr;
 }
 
-template <int BN, int STAGES, int EPI, int ACT, bool CONV, bool PAIR = false>
-static int configure_inst() {
-  auto kern = gemm_wgmma_kernel<BN, STAGES, EPI, ACT, CONV, PAIR>;
-  constexpr size_t smem = gemm_smem_bytes<BN, STAGES>();
-  if (int rc = check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem),
-                          "cudaFuncSetAttribute(gemm smem)"))
-    return rc;
-  cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-  return 0;
-}
-
-#define F5_GEMM_CASE(BN_, ST_, EPI_, ACT_, CONV_)                                                                   \
-  if (!pl.pair && pl.bn == BN_ && pl.epi == EPI_ && pl.act == ACT_ && (pl.conv != 0) == CONV_)        \
-    return launch_inst<BN_, ST_, EPI_, ACT_, CONV_>(pl, s);
-#define F5_GEMM_PAIR_CASE(BN_, ST_, EPI_, ACT_)                                                  \
-  if (pl.pair && pl.bn == BN_ && pl.epi == EPI_ && pl.act == ACT_ && !pl.conv)     \
-    return launch_inst<BN_, ST_, EPI_, ACT_, false, true>(pl, s);
 // cudaFuncSetAttribute is per device: the configured flag and the SM count are tracked per device ordinal, so one
 // process may drive engines on several GPUs (ADVICE r1).
 namespace {
@@ -130,41 +135,13 @@ int configure_kernels() {
   const int dev = current_device();
   std::lock_guard<std::mutex> lk(g_dev_mu);
   if (g_dev[dev].configured) return 0;
-  if (int rc = configure_inst<64, 7, EPI_F16, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<64, 7, EPI_F16, ACT_GELU_TANH, false>()) return rc;
-  if (int rc = configure_inst<64, 7, EPI_F16, ACT_GELU_ERF, false>()) return rc;
-  if (int rc = configure_inst<64, 7, EPI_F32, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<64, 7, EPI_RESID, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<128, 5, EPI_F16, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<128, 5, EPI_F16, ACT_GELU_TANH, false>()) return rc;
-  if (int rc = configure_inst<128, 5, EPI_F16, ACT_GELU_ERF, false>()) return rc;
-  if (int rc = configure_inst<128, 5, EPI_F32, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<128, 5, EPI_RESID, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<256, 3, EPI_F16, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<256, 3, EPI_F16, ACT_GELU_TANH, false>()) return rc;
-  if (int rc = configure_inst<256, 3, EPI_F16, ACT_GELU_ERF, false>()) return rc;
-  if (int rc = configure_inst<256, 3, EPI_F32, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<256, 3, EPI_RESID, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<128, 5, EPI_QKV_ROPE, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<192, 4, EPI_QKV_ROPE, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<192, 4, EPI_F16, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<192, 4, EPI_F16, ACT_GELU_TANH, false>()) return rc;
-  if (int rc = configure_inst<192, 4, EPI_RESID, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<256, 3, EPI_QKV_ROPE, ACT_NONE, false>()) return rc;
-  if (int rc = configure_inst<64, 7, EPI_F16, ACT_MISH, true>()) return rc;
-  if (int rc = configure_inst<64, 7, EPI_RESID, ACT_MISH, true>()) return rc;
-  if (int rc = configure_inst<256, 4, EPI_F16, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<256, 4, EPI_F16, ACT_GELU_TANH, false, true>()) return rc;
-  if (int rc = configure_inst<256, 4, EPI_RESID, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<256, 4, EPI_QKV_ROPE, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<192, 5, EPI_F16, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<192, 5, EPI_F16, ACT_GELU_TANH, false, true>()) return rc;
-  if (int rc = configure_inst<192, 5, EPI_RESID, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<192, 5, EPI_QKV_ROPE, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<128, 6, EPI_F16, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<128, 6, EPI_F16, ACT_GELU_TANH, false, true>()) return rc;
-  if (int rc = configure_inst<128, 6, EPI_RESID, ACT_NONE, false, true>()) return rc;
-  if (int rc = configure_inst<128, 6, EPI_QKV_ROPE, ACT_NONE, false, true>()) return rc;
+  for (const GemmKernel& k : kGemmKernels) {
+    if (int rc = check_cuda(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)gemm_smem_bytes(k.bn)),
+                            "cudaFuncSetAttribute(gemm smem)"))
+      return rc;
+    cudaFuncSetAttribute(k.fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+  }
   if (int rc = attn_configure()) return rc;
   g_dev[dev].configured = true;
   return 0;
@@ -194,99 +171,69 @@ int num_sms() {
 }
 
 int gemm_run(const GemmPlan& pl, cudaStream_t s) {
-  F5_GEMM_CASE(64, 7, EPI_F16, ACT_NONE, false)
-  F5_GEMM_CASE(64, 7, EPI_F16, ACT_GELU_TANH, false)
-  F5_GEMM_CASE(64, 7, EPI_F16, ACT_GELU_ERF, false)
-  F5_GEMM_CASE(64, 7, EPI_F32, ACT_NONE, false)
-  F5_GEMM_CASE(64, 7, EPI_RESID, ACT_NONE, false)
-  F5_GEMM_CASE(128, 5, EPI_F16, ACT_NONE, false)
-  F5_GEMM_CASE(128, 5, EPI_F16, ACT_GELU_TANH, false)
-  F5_GEMM_CASE(128, 5, EPI_F16, ACT_GELU_ERF, false)
-  F5_GEMM_CASE(128, 5, EPI_F32, ACT_NONE, false)
-  F5_GEMM_CASE(128, 5, EPI_RESID, ACT_NONE, false)
-  F5_GEMM_CASE(256, 3, EPI_F16, ACT_NONE, false)
-  F5_GEMM_CASE(256, 3, EPI_F16, ACT_GELU_TANH, false)
-  F5_GEMM_CASE(256, 3, EPI_F16, ACT_GELU_ERF, false)
-  F5_GEMM_CASE(256, 3, EPI_F32, ACT_NONE, false)
-  F5_GEMM_CASE(256, 3, EPI_RESID, ACT_NONE, false)
-  F5_GEMM_CASE(128, 5, EPI_QKV_ROPE, ACT_NONE, false)
-  F5_GEMM_CASE(192, 4, EPI_QKV_ROPE, ACT_NONE, false)
-  F5_GEMM_CASE(192, 4, EPI_F16, ACT_NONE, false)
-  F5_GEMM_CASE(192, 4, EPI_F16, ACT_GELU_TANH, false)
-  F5_GEMM_CASE(192, 4, EPI_RESID, ACT_NONE, false)
-  F5_GEMM_CASE(256, 3, EPI_QKV_ROPE, ACT_NONE, false)
-  F5_GEMM_CASE(64, 7, EPI_F16, ACT_MISH, true)
-  F5_GEMM_CASE(64, 7, EPI_RESID, ACT_MISH, true)
-  F5_GEMM_PAIR_CASE(256, 4, EPI_F16, ACT_NONE)
-  F5_GEMM_PAIR_CASE(256, 4, EPI_F16, ACT_GELU_TANH)
-  F5_GEMM_PAIR_CASE(256, 4, EPI_RESID, ACT_NONE)
-  F5_GEMM_PAIR_CASE(256, 4, EPI_QKV_ROPE, ACT_NONE)
-  F5_GEMM_PAIR_CASE(192, 5, EPI_F16, ACT_NONE)
-  F5_GEMM_PAIR_CASE(192, 5, EPI_F16, ACT_GELU_TANH)
-  F5_GEMM_PAIR_CASE(192, 5, EPI_RESID, ACT_NONE)
-  F5_GEMM_PAIR_CASE(192, 5, EPI_QKV_ROPE, ACT_NONE)
-  F5_GEMM_PAIR_CASE(128, 6, EPI_F16, ACT_NONE)
-  F5_GEMM_PAIR_CASE(128, 6, EPI_F16, ACT_GELU_TANH)
-  F5_GEMM_PAIR_CASE(128, 6, EPI_RESID, ACT_NONE)
-  F5_GEMM_PAIR_CASE(128, 6, EPI_QKV_ROPE, ACT_NONE)
-  set_error("gemm: no kernel instantiated for bn=%d epi=%d act=%d conv=%d pair=%d", pl.bn, pl.epi, pl.act, pl.conv, pl.pair);
-  return -6;
+  const GemmKernel* k = find_kernel(pl.bn, pl.epi, pl.act, pl.conv != 0);
+  if (!k) {
+    set_error("gemm: no kernel instantiated for bn=%d epi=%d act=%d conv=%d", pl.bn, pl.epi, pl.act, pl.conv);
+    return -6;
+  }
+  if (int rc = configure_kernels()) return rc;
+  PdlLaunch L(pl.grid, dim3(kGemmThreads), gemm_smem_bytes(pl.bn), s);
+  if (int rc = check_cuda(cudaLaunchKernelEx(&L.cfg, k->fn, pl.tmA, pl.tmB, pl.p), "gemm launch")) return rc;
+  count_launch();
+  return check_launch("gemm_wgmma_kernel launch");
 }
 
-struct TileChoice {
-  int bn, pair;
-};
-// Tile shape of a GEMM whose caller left bn = 0.  Cost model in SM clocks of the H100 (132 SMs, 4096 dense fp16
+// Tile width of a GEMM whose caller left bn = 0.  Cost model in SM clocks of the H100 (132 SMs, 4096 dense fp16
 // FLOP / clk / SM): the wgmma main loop of a 128 x BN tile takes k-blocks x (4 BN + 96) clk (tensor-core time plus the
 // per-k-block barrier and issue overhead), the register epilogue BN x {20 plain / RoPE, 24 reduce-add, 32 GELU} clk.
 // Tiles run in rounds over the SMs; the producer streams the next tile's operands during the epilogue, so a round
 // costs main + epilogue.  Checked against the graph-timed sweep of tools/gemm_sweep.py with the chunked epilogue (H100
-// SXM 80 GB, 700 W limit): the pick is the fastest width at M = 1876 and within 11 % of it at M = 3752 - 15008.  Cluster
-// pairs (cta_pair = 1) were 1.6 - 3.8x slower than single-CTA tiles in every row of that sweep, so they are never picked.
-// Diagnostic build (make TRACE=1) only: F5_BN_<n_out>=<bn>[p] overrides the choice.
-TileChoice pick_tile(long long rows, int batches, int n_out, int k, int epi, int act) {
+// SXM 80 GB, 700 W limit): the pick is the fastest width at M = 1876 and within 11 % of it at M = 3752 - 15008.
+// Diagnostic build (make TRACE=1) only: F5_BN_<n_out>=<bn> overrides the choice.
+static int pick_tile(long long rows, int batches, int n_out, int k, int epi, int act) {
 #ifdef F5_TRACE
   char key[32];
   snprintf(key, sizeof key, "F5_BN_%d", n_out);
   if (const char* e = getenv(key)) {
     const int bn = atoi(e);
-    if (bn == 64 || bn == 128 || bn == 192 || bn == 256) return {bn, strchr(e, 'p') != nullptr ? 1 : 0};
+    if (bn == 64 || bn == 128 || bn == 192 || bn == 256) return bn;
   }
 #endif
   const int sms = num_sms();
   const double kb = double((k + 63) / 64);
   const double epi_col = (act == F5_ACT_GELU_TANH || act == F5_ACT_GELU_ERF) ? 32.0 : (epi == F5_EPI_RESID ? 24.0 : 20.0);
-  // instantiated combinations only (configure_kernels)
-  const bool plain = act == F5_ACT_NONE, gelu = epi == F5_EPI_F16 && act == F5_ACT_GELU_TANH;
-  const bool wide_ok = (epi == F5_EPI_F16 && (plain || gelu)) || ((epi == F5_EPI_RESID || epi == F5_EPI_QKV_ROPE) && plain);
-  TileChoice best{128, 0};
+  int best = 128;
   double best_cost = 1e30;
   const int cand[3] = {128, 192, 256};
   for (const int bn : cand) {
-    if (bn == 192 && !wide_ok) continue;
+    if (!find_kernel(bn, epi, act, false)) continue;
     if (bn > 128 && n_out < bn) continue;
     const long long tiles = ((rows + 127) / 128) * ((n_out + bn - 1) / bn) * batches;
     const double rounds = double((tiles + sms - 1) / sms);
     const double cost = rounds * (kb * (4.0 * bn + 96.0) + epi_col * bn);
     if (cost < best_cost) {
       best_cost = cost;
-      best = {bn, 0};
+      best = bn;
     }
   }
   return best;
 }
 
+// Tile width f5_gemm runs `a` with: conv tiles are 64 wide, bn = 0 leaves the width to the planner.
+static int resolve_tile(const f5_gemm_args* a, int* bn) {
+  if (a->cta_pair != 0) {
+    set_error("gemm: cta_pair must be 0 (there are no cluster-pair tiles)");
+    return -1;
+  }
+  *bn = a->conv_taps > 0 ? 64 : a->bn != 0 ? a->bn : pick_tile(a->rows, a->batches, a->n_out, a->k, a->epi, a->act);
+  return 0;
+}
+
 int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a) {
   memset(pl, 0, sizeof(*pl));
   const bool conv = a->conv_taps > 0;
-  int bn = a->bn;
-  int want_pair = a->cta_pair;
-  if (conv) bn = 64;
-  if (bn == 0) {  // caller leaves the tile shape to the planner
-    const TileChoice tc = pick_tile(a->rows, a->batches, a->n_out, a->k, a->epi, a->act);
-    bn = tc.bn;
-    want_pair = tc.pair;
-  }
+  int bn;
+  if (int rc = resolve_tile(a, &bn)) return rc;
   if (bn != 64 && bn != 128 && bn != 192 && bn != 256) {
     set_error("gemm: bn must be 64, 128, 192 or 256");
     return -1;
@@ -303,7 +250,6 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
   pl->epi = a->epi;
   pl->act = a->act;
   pl->conv = conv ? 1 : 0;
-  pl->pair = (!conv && want_pair && a->epi != F5_EPI_F32 && bn >= 128) ? 1 : 0;
   GemmParams& p = pl->p;
   p.rows = a->rows;
   p.n_out = a->n_out;
@@ -354,8 +300,8 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     rc = encode_tmap_f16(&pl->tmA, A, (uint64_t)a->k, (uint64_t)a->rows, (uint64_t)a->batches, (uint64_t)a->lda * 2,
                          (uint64_t)a->rows * a->lda * 2, 64, 128, 3);
     if (rc) return rc;
-    rc = encode_tmap_f16(&pl->tmB, W, (uint64_t)a->k, (uint64_t)a->n_out, 1, (uint64_t)a->ldw * 2, 0, 64,
-                         (uint32_t)(pl->pair ? bn / 2 : bn), 2);
+    rc = encode_tmap_f16(&pl->tmB, W, (uint64_t)a->k, (uint64_t)a->n_out, 1, (uint64_t)a->ldw * 2, 0, 64, (uint32_t)bn,
+                         2);
     if (rc) return rc;
   }
   if (a->epi == F5_EPI_RESID && (a->ldo % 4 || a->resid == nullptr)) {
@@ -366,12 +312,6 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     set_error("gemm: fp16 epilogue needs out != NULL and ldo %% 8 == 0 (ldo=%d)", a->ldo);
     return -1;
   }
-  if (pl->pair) {
-    const long long ptiles = (long long)((a->n_out + bn - 1) / bn) * ((a->rows + 2 * kBM - 1) / (2 * kBM)) * a->batches;
-    const long long pairs = num_sms() / 2;
-    pl->grid = dim3((unsigned)(2 * (ptiles < pairs ? ptiles : pairs)), 1, 1);  // persistent CTA pairs
-    return 0;
-  }
   const long long tiles = (long long)((a->n_out + bn - 1) / bn) * ((a->rows + kBM - 1) / kBM) * a->batches;
   pl->grid = dim3((unsigned)(tiles < num_sms() ? tiles : num_sms()), 1, 1);  // persistent: one CTA per SM
   return 0;
@@ -381,21 +321,14 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 
 extern "C" {
 
-int f5_version(void) { return 101; }
+int f5_version(void) { return 102; }
 const char* f5_last_error(void) { return f5::g_err; }
 unsigned long long f5_launch_count(void) { return f5::g_launches.load(); }
 
 int f5_gemm_tile(const f5_gemm_args* args, int* bn, int* cta_pair) {
   if (!args || !bn || !cta_pair) return -1;
-  int b = args->conv_taps > 0 ? 64 : args->bn, pr = args->cta_pair;
-  if (b == 0) {
-    const f5::TileChoice tc = f5::pick_tile(args->rows, args->batches, args->n_out, args->k, args->epi, args->act);
-    b = tc.bn;
-    pr = tc.pair;
-  }
-  *bn = b;
-  *cta_pair = (args->conv_taps == 0 && pr && args->epi != F5_EPI_F32 && b >= 128) ? 1 : 0;
-  return 0;
+  *cta_pair = 0;
+  return f5::resolve_tile(args, bn);
 }
 
 int f5_gemm(const void* A, const void* W, const f5_gemm_args* args, f5_stream_t stream) {

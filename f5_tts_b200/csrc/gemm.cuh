@@ -26,9 +26,11 @@ namespace f5 {
 constexpr int kGemmThreads = 288;  // two consumer warpgroups + one producer warp
 constexpr int kGemmEmptyArrivals = 8;  // consumer warps per CTA
 
-template <int BN, int STAGES>
-constexpr size_t gemm_smem_bytes() {
-  return size_t(STAGES) * (kBM * kBK * 2 + BN * kBK * 2) + 1024 /*align slack*/ + 256 /*barriers*/;
+// depth of the {A, W} k-block ring for a BN-wide tile
+__host__ __device__ constexpr int gemm_stages(int bn) { return bn == 64 ? 7 : bn == 128 ? 5 : bn == 192 ? 4 : 3; }
+
+constexpr size_t gemm_smem_bytes(int bn) {
+  return size_t(gemm_stages(bn)) * (kBM * kBK * 2 + bn * kBK * 2) + 1024 /*align slack*/ + 256 /*barriers*/;
 }
 
 template <int BN>
@@ -41,13 +43,13 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[BN / 2], uint64_t da, uint
 
 // Packed / variable-length execution (SURVEY.md §8f-1; reference masked mode modules.py:513-540): with skip_pad, a tile
 // whose rows ALL lie past the end of their sample is never loaded, multiplied or stored.  Every warp role evaluates the
-// same predicate, so the smem ring and the tile order stay in step.  m0 = first row of the (pair-)tile, tm = its height;
+// same predicate, so the smem ring and the tile order stay in step.  m0 = first row of the tile;
 // CONV: rows are per sample (bz), plain: rows are the flattened [samples x seq] axis.
 template <bool CONV>
-__device__ __forceinline__ bool tile_is_padding(const GemmParams& p, int m0, int tm, int bz) {
+__device__ __forceinline__ bool tile_is_padding(const GemmParams& p, int m0, int bz) {
   if (!p.skip_pad) return false;
   if (CONV) return m0 >= p.row_len[bz];
-  const int last = min(m0 + tm, p.rows) - 1;
+  const int last = min(m0 + kBM, p.rows) - 1;
   const int b0 = m0 / p.seq;
   if (b0 != last / p.seq) return false;  // the tile reaches into the next sample, whose first rows are valid
   return m0 - b0 * p.seq >= p.row_len[b0];
@@ -205,17 +207,11 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
   }
 }
 
-// PAIR = true: a cluster of two CTAs computes one 256 x BN tile, each CTA its own 128 rows.  Each CTA loads HALF of the
-// W tile (BN/2 rows) and multicasts it into both CTAs' rings, so the pair reads W from L2 once instead of twice.  A ring
-// slot is refilled only after the consumers of BOTH CTAs released it (empty barriers count the peer's warps as well).
-template <int BN, int STAGES, int EPI, int ACT, bool CONV, bool PAIR = false>
+template <int BN, int EPI, int ACT, bool CONV>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  static_assert(!(PAIR && CONV), "the conv schedule is single-CTA");
   static_assert(BN == 64 || BN == 128 || BN == 192 || BN == 256, "BN");
-  static_assert(!(PAIR && BN == 64), "pair tiles are 128, 192 or 256 wide");
-  constexpr int BNL = PAIR ? BN / 2 : BN;   // W rows loaded by this CTA
-  constexpr int TM = PAIR ? 2 * kBM : kBM;  // rows of one (pair-)tile
+  constexpr int STAGES = gemm_stages(BN);
   constexpr uint32_t A_BYTES = kBM * kBK * 2;
   constexpr uint32_t B_BYTES = BN * kBK * 2;
 
@@ -228,11 +224,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x >> 5;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
-  const int cta_id = PAIR ? int(blockIdx.x >> 1) : int(blockIdx.x);
-  const int cta_step = PAIR ? int(gridDim.x >> 1) : int(gridDim.x);
+  const int cta_id = int(blockIdx.x);
+  const int cta_step = int(gridDim.x);
   const int tiles_n = (p.n_out + BN - 1) / BN;
-  const int tiles_m = (p.rows + TM - 1) / TM;
+  const int tiles_m = (p.rows + kBM - 1) / kBM;
   const int num_tiles = tiles_n * tiles_m * p.batches;
 
   if (warp == 8 && elect_one()) {
@@ -240,12 +235,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], (PAIR ? 2 : 1) * kGemmEmptyArrivals);
+      mbar_init(&empty[s], kGemmEmptyArrivals);
     }
     fence_mbar_init();
   }
-  if (PAIR) cluster_sync_all();  // the peer's barriers are initialised before any multicast or remote arrive
-  else __syncthreads();
+  __syncthreads();
   // Programmatic dependent launch: everything above overlapped the predecessor's tail.  The producer goes one step
   // further (below): W tiles are weights, not produced by the predecessor, so their TMA loads are issued BEFORE the
   // dependency wait and the DRAM latency of the first STAGES k-blocks hides under the predecessor too.
@@ -257,9 +251,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // ===== TMA producer =====
       uint32_t it = 0;  // running k-block counter across tiles -> stage / phase
       auto load_w = [&](int s, int kb, int n0) {
-        if (PAIR)
-          tma_load_2d_multicast(sB + s * B_BYTES + rank * (BNL * 128), &tmB, &full[s], kb * kBK, n0 + int(rank) * BNL, 3);
-        else if (CONV) tma_load_2d(sB + s * B_BYTES, &tmB, &full[s], 0, kb * p.n_out + n0);  // [tap][out_channel][in 64]
+        if (CONV) tma_load_2d(sB + s * B_BYTES, &tmB, &full[s], 0, kb * p.n_out + n0);  // [tap][out_channel][in 64]
         else tma_load_2d(sB + s * B_BYTES, &tmB, &full[s], kb * kBK, n0);
       };
       // weights of the first tile's first k-blocks: in flight before the dependency wait (slots are free at start)
@@ -274,15 +266,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       pdl_wait();
       for (int t = cta_id; t < num_tiles; t += cta_step) {
         const int n0 = (t % tiles_n) * BN;
-        const int m0 = ((t / tiles_n) % tiles_m) * TM + int(rank) * kBM;
+        const int m0 = ((t / tiles_n) % tiles_m) * kBM;
         const int bz = t / (tiles_n * tiles_m);
-        if (tile_is_padding<CONV>(p, ((t / tiles_n) % tiles_m) * TM, TM, bz)) continue;
+        if (tile_is_padding<CONV>(p, m0, bz)) continue;
         for (int kb = 0; kb < p.num_kb; ++kb, ++it) {
           const int s = it % STAGES;
           const uint32_t ph = (it / STAGES) & 1;
           if (it >= pre) {
             mbar_wait(&empty[s], ph ^ 1);
-            mbar_expect_tx(&full[s], A_BYTES + B_BYTES);  // PAIR: the peer's W half lands here as well
+            mbar_expect_tx(&full[s], A_BYTES + B_BYTES);
             load_w(s, kb, n0);
           }
           if (CONV) tma_load_3d(sA + s * A_BYTES, &tmA, &full[s], n0, m0 + kb - p.conv_pad, bz);  // tap shift
@@ -302,20 +294,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     float acc[BN / 2];
     uint32_t it = 0;
     auto release = [&](int s) {
-      if (lane == 0) {
-        if (PAIR) {
-          mbar_arrive_cluster(&empty[s], 0);
-          mbar_arrive_cluster(&empty[s], 1);
-        } else {
-          mbar_arrive(&empty[s]);
-        }
-      }
+      if (lane == 0) mbar_arrive(&empty[s]);
     };
     for (int t = cta_id; t < num_tiles; t += cta_step) {
       const int n0 = (t % tiles_n) * BN;
-      const int m0 = ((t / tiles_n) % tiles_m) * TM + int(rank) * kBM;
+      const int m0 = ((t / tiles_n) % tiles_m) * kBM;
       const int bz = t / (tiles_n * tiles_m);
-      if (tile_is_padding<CONV>(p, ((t / tiles_n) % tiles_m) * TM, TM, bz)) continue;
+      if (tile_is_padding<CONV>(p, m0, bz)) continue;
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb, ++it) {
         const int s = it % STAGES;
@@ -341,7 +326,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       epilogue_tile<BN, EPI, ACT>(p, acc, n0, c2, m0 + r_in_tile, bz, gate);
     }
   }
-  if (PAIR) cluster_sync_all();  // the peer may still be multicasting into our smem / arriving on our barriers
 }
 
 }  // namespace f5

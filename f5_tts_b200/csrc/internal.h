@@ -21,28 +21,17 @@ bool pdl_enabled();  // F5_PDL=0 disables programmatic dependent launch
 // griddepcontrol.wait before touching global memory, so stream order is preserved transitively.
 struct PdlLaunch {
   cudaLaunchConfig_t cfg;
-  cudaLaunchAttribute attr[2];
-  PdlLaunch(dim3 grid, dim3 block, size_t smem, cudaStream_t s, int cluster_x = 1) {
+  cudaLaunchAttribute attr;
+  PdlLaunch(dim3 grid, dim3 block, size_t smem, cudaStream_t s) {
     cfg = cudaLaunchConfig_t{};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = s;
-    int n = 0;
-    if (cluster_x > 1) {  // CTA pair for cta_group::2 kernels
-      attr[n].id = cudaLaunchAttributeClusterDimension;
-      attr[n].val.clusterDim.x = (unsigned)cluster_x;
-      attr[n].val.clusterDim.y = 1;
-      attr[n].val.clusterDim.z = 1;
-      ++n;
-    }
-    if (pdl_enabled()) {
-      attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[n].val.programmaticStreamSerializationAllowed = 1;
-      ++n;
-    }
-    cfg.attrs = attr;
-    cfg.numAttrs = n;
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = pdl_enabled() ? 1 : 0;
   }
 };
 
@@ -50,7 +39,7 @@ struct GemmPlan {
   CUtensorMap tmA, tmB;
   GemmParams p;
   dim3 grid;
-  int bn, epi, act, conv, pair;
+  int bn, epi, act, conv;
 };
 int gemm_plan(GemmPlan* plan, const void* A, const void* W, const f5_gemm_args* a);
 int gemm_run(const GemmPlan& plan, cudaStream_t s);
@@ -65,8 +54,6 @@ int attn_plan(AttnPlan* plan, const void* qkv, void* out, int batches, int seq, 
 int attn_run(const AttnPlan& plan, cudaStream_t s);
 
 // 3-D fp16 tensor map: dims (d0 contiguous, d1, d2), byte strides for d1, d2, box (b0, b1, 1), 128B swizzle
-int encode_tmap(CUtensorMap* m, int is_f32, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
-                uint64_t stride2, uint32_t b0, uint32_t b1, int rank);
 int encode_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                     uint64_t stride2, uint32_t b0, uint32_t b1, int rank);
 

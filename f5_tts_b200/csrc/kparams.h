@@ -34,7 +34,7 @@ struct GemmParams {
   int inner;     // heads * dim_head
   int pe_heads;  // heads that get rotary (q and k sections)
   int conv_pad;  // CONV: taps/2
-  int skip_pad;    // 1: 128-row (256 for CTA pairs) tiles whose rows all lie past their sample's row_len are not computed
+  int skip_pad;    // 1: 128-row tiles whose rows all lie past their sample's row_len are not computed
   int w_prefetch;  // W tiles may be loaded before griddepcontrol.wait (weights are not produced by the predecessor)
 #ifdef F5_TRACE
   int diag_no_epi;  // instrumented build: skip the epilogue (nothing is stored) to time the main loop alone

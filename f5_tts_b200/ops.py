@@ -70,7 +70,7 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, epi=EPI_F16, act=ACT_
 
 
 def gemm_tile(M: int, N: int, K: int, epi=EPI_F16, act=ACT_NONE, bn=0, pair=0):
-    """(tile width, cta_pair) the planner runs this GEMM shape with."""
+    """(tile width, cta_pair) the planner runs this GEMM shape with; cta_pair is always 0 (a non-zero `pair` raises)."""
     g = _lib.GemmArgs()
     g.rows, g.batches, g.n_out, g.k, g.bn, g.epi, g.act, g.cta_pair = M, 1, N, K, bn, epi, act, pair
     b, pr = C.c_int(0), C.c_int(0)

@@ -12,7 +12,7 @@
  * The reference has no native FFI on this path (it is pure PyTorch); the binding a maintainer adds is the ctypes
  * stub shown in INTEGRATION.md / f5_tts_b200/_lib.py.
  *
- * Requires an sm_90a device (wgmma / TMA / clusters).  There is no CPU or non-Hopper fallback.
+ * Requires an sm_90a device (wgmma / TMA).  There is no CPU or non-Hopper fallback.
  */
 #ifndef F5TTS_B200_H
 #define F5TTS_B200_H
@@ -48,10 +48,10 @@ typedef struct {
   int n_out;
   int k;         /* reduction length (plain) ; ignored for conv */
   int lda, ldw;  /* elements */
-  int bn;        /* output tile width: 64 | 128 | 192 | 256 (0 = the planner picks width and cta_pair) */
+  int bn;        /* output tile width: 64 | 128 | 192 | 256 (0 = the planner picks the width) */
   int epi, act;
   int conv_taps; /* 0 = plain GEMM */
-  int cta_pair;  /* 1 = 256 x bn tiles on a 2-CTA cluster sharing W by multicast; bn 128, 192 or 256; plain GEMM, not EPI_F32 */
+  int cta_pair;  /* must be 0 (there are no cluster-pair tiles); kept so the struct layout does not change */
   const float* bias;
   void* out;               /* fp16 (F16 / QKV_ROPE) or fp32 (F32) [batches*rows, ldo] */
   void* out16b;            /* optional fp16 masked copy for F32 */
@@ -73,7 +73,7 @@ typedef struct {
   int skip_padded_tiles;
 } f5_gemm_args;
 int f5_gemm(const void* A, const void* W, const f5_gemm_args* args, f5_stream_t stream);
-/* Tile shape f5_gemm would run `args` with (after bn = 0 resolution): *bn tile width, *cta_pair 0/1. */
+/* Tile shape f5_gemm would run `args` with (after bn = 0 resolution): *bn tile width, *cta_pair always 0. */
 int f5_gemm_tile(const f5_gemm_args* args, int* bn, int* cta_pair);
 
 /* Non-causal attention over the fused QKV buffer — replaces F.scaled_dot_product_attention at

@@ -16,7 +16,7 @@ pytestmark = pytest.mark.gpu
 if not torch.cuda.is_available():
     pytest.skip("needs a CUDA device", allow_module_level=True)
 
-from f5_tts_b200 import ops  # noqa: E402
+from f5_tts_b200 import _lib, ops  # noqa: E402
 from f5_tts_b200.ops import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_NONE, EPI_F16, EPI_F32, EPI_QKV_ROPE,  # noqa: E402
                              EPI_RESID)
 
@@ -52,25 +52,33 @@ def test_gemm_f32(M, N, K, bn):
 @pytest.mark.parametrize("M,N,K,bn", [(256, 256, 64, 256), (1876, 2048, 1024, 256), (1876, 3072, 1024, 128), (700, 1024, 2048, 128),
                                       (129, 512, 192, 256), (30000 // 8, 2048, 1024, 256), (1876, 3072, 1024, 192),
                                       (500, 1024, 2048, 192)])
-def test_gemm_cta_pair(M, N, K, bn):
-    """Cluster-pair tiles (256 x bn per 2-CTA cluster, W multicast): fp16+GELU, fp32 residual add and QKV+RoPE epilogues."""
+def test_gemm_wide_tiles(M, N, K, bn):
+    """128-, 192- and 256-wide tiles, including M not a multiple of 128 and K = 2048: fp16+GELU, fp32 residual add and
+    QKV+RoPE epilogues."""
     a, w = gen((M, K), 31), gen((N, K), 32, 1 / math.sqrt(K))
     bias = gen((N,), 33, 0.5, torch.float32)
     ref = a.float() @ w.float().t() + bias
-    out = ops.linear(a, w, bias, epi=EPI_F16, act=ACT_GELU_TANH, bn=bn, pair=1)
-    report(f"pair f16 gelu {M}x{N}x{K} bn{bn}", out, F.gelu(ref, approximate="tanh"))
+    out = ops.linear(a, w, bias, epi=EPI_F16, act=ACT_GELU_TANH, bn=bn)
+    report(f"f16 gelu {M}x{N}x{K} bn{bn}", out, F.gelu(ref, approximate="tanh"))
     assert rel(out, F.gelu(ref, approximate="tanh")) <= 1.5e-3
     x0 = gen((M, N), 34, 1.0, torch.float32)
     gate = gen((N,), 35, 0.5, torch.float32)
     x = x0.clone()
-    ops.linear(a, w, bias, epi=EPI_RESID, bn=bn, pair=1, resid=x, gate=gate)
+    ops.linear(a, w, bias, epi=EPI_RESID, bn=bn, resid=x, gate=gate)
     assert rel(x, x0 + gate * ref) <= 2e-4
     if N % 192 == 0:
         seq, inner = M // 2, N // 3
         cs, sn = ops.rope_tables(seq, DEV)
-        o = ops.linear(a[: 2 * seq], w, bias, epi=EPI_QKV_ROPE, bn=bn, pair=1, seq=seq, rope=(cs, sn), inner=inner, pe_heads=1)
+        o = ops.linear(a[: 2 * seq], w, bias, epi=EPI_QKV_ROPE, bn=bn, seq=seq, rope=(cs, sn), inner=inner, pe_heads=1)
         o1 = ops.linear(a[: 2 * seq], w, bias, epi=EPI_QKV_ROPE, bn=128, seq=seq, rope=(cs, sn), inner=inner, pe_heads=1)
-        assert rel(o, o1) <= 1e-6  # same arithmetic as the single-CTA kernel
+        assert rel(o, o1) <= 1e-6  # the tile width does not change the arithmetic
+
+
+def test_gemm_rejects_cta_pair():
+    """There are no cluster-pair tiles: a request for one is an error, not a silent single-CTA run."""
+    a, w = gen((256, 128), 36), gen((256, 128), 37)
+    with pytest.raises(_lib.F5LibraryError):
+        ops.linear(a, w, epi=EPI_F16, bn=128, pair=1)
 
 
 @pytest.mark.parametrize("act", [ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF])

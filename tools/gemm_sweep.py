@@ -19,11 +19,11 @@ torch.cuda.init()
 g = torch.Generator().manual_seed(0)
 
 
-def bench(M, N, K, epi, act, bn, nw=24, pair=0):
+def bench(M, N, K, epi, act, bn, nw=24):
     a = [torch.randn(M, K, generator=g).half().to(DEV) for _ in range(2)]
     w = [(torch.randn(N, K, generator=g) / 32).half().to(DEV) for _ in range(nw)]
     b = torch.randn(N, generator=g).to(DEV)
-    kw = dict(epi=epi, act=act, bn=bn, pair=pair, static_w=True)
+    kw = dict(epi=epi, act=act, bn=bn, static_w=True)
     if epi == EPI_RESID:
         kw["resid"] = torch.zeros(M, N, device=DEV)
         kw["gate"] = torch.randn(N, generator=g).to(DEV)
@@ -50,11 +50,10 @@ for M in Ms:
             continue
         nw = -(-200_000_000 // (N * K * 2))  # distinct weights > L2 (50 MB), as in the real step
         nw = nw if M < 8000 else max(6, nw // 4)
-        auto = ops.gemm_tile(M, N, K, epi, act)
-        tiles = [(auto[0], auto[1])] if pick_only else ((128, 0), (192, 0), (256, 0), (128, 1), (192, 1), (256, 1))
+        auto = ops.gemm_tile(M, N, K, epi, act)[0]
         row = []
-        for bn, pair in tiles:
-            us, tf = bench(M, N, K, epi, act, bn, nw=nw, pair=pair)
-            row.append(f"{'P' if pair else 'bn'}{bn}: {us:6.1f}us {tf:5.0f}TF")
+        for bn in [auto] if pick_only else (128, 192, 256):
+            us, tf = bench(M, N, K, epi, act, bn, nw=nw)
+            row.append(f"bn{bn}: {us:6.1f}us {tf:5.0f}TF")
         print(f"M={M:6d} {tag:7s} N={N:5d} K={K:5d} | " + " | ".join(row) + f" | auto={auto}"
               f" | cuBLAS {cublas(M, N, K, nw):6.1f}us", flush=True)
