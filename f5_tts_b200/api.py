@@ -1,8 +1,8 @@
 """``F5TTS`` — mirror of the reference's top-level API class (f5_tts/api.py:23-149) over the H100 sampler.
 
 Same constructor / ``infer`` signature and return value ``(wav np.float32[nw], sr, spec np[100, n])``.  Differences,
-all forced by the offline image and the scope of this build: model configs are the three shipped architectures
-hard-coded below (hydra/omegaconf are not installed; values copied from configs/*.yaml ``model.arch``); checkpoints
+all forced by the offline image and the scope of this build: model configs are the six shipped architectures
+(Base and Small of F5TTS_v1, F5TTS and E2TTS) hard-coded below (hydra/omegaconf are not installed; values copied from configs/*.yaml ``model.arch``); checkpoints
 and the vocoder must be given as local paths (no network); ``transcribe`` and silence removal are not mirrored.
 """
 from __future__ import annotations
@@ -25,6 +25,15 @@ MODEL_ARCH = {
                             conv_layers=4, pe_attn_head=1, attn_backend="torch", attn_mask_enabled=False)),
     # configs/E2TTS_Base.yaml:25-31
     "E2TTS_Base": (UNetT, dict(dim=1024, depth=24, heads=16, ff_mult=4, text_mask_padding=False, pe_attn_head=1)),
+    # configs/F5TTS_v1_Small.yaml:26-36
+    "F5TTS_v1_Small": (DiT, dict(dim=768, depth=18, heads=12, ff_mult=2, text_dim=512, text_mask_padding=True,
+                                qk_norm=None, conv_layers=4, pe_attn_head=None, attn_backend="torch",
+                                attn_mask_enabled=False)),
+    # configs/F5TTS_Small.yaml:25-35
+    "F5TTS_Small": (DiT, dict(dim=768, depth=18, heads=12, ff_mult=2, text_dim=512, text_mask_padding=False,
+                             conv_layers=4, pe_attn_head=1, attn_backend="torch", attn_mask_enabled=False)),
+    # configs/E2TTS_Small.yaml:25-31
+    "E2TTS_Small": (UNetT, dict(dim=768, depth=20, heads=12, ff_mult=4, text_mask_padding=False, pe_attn_head=1)),
 }
 
 

@@ -11,8 +11,10 @@ int attn_plan(AttnPlan* pl, const void* qkv, void* out, int batches, int seq, in
     return -1;
   }
   const int inner = heads * 64;
-  int rc = encode_tmap_f16(&pl->tm, qkv, (uint64_t)3 * inner, (uint64_t)seq, (uint64_t)batches, (uint64_t)3 * inner * 2,
-                           (uint64_t)seq * 3 * inner * 2, 64, 128, 3);
+  const uint64_t dims[3] = {(uint64_t)3 * inner, (uint64_t)seq, (uint64_t)batches};
+  const uint64_t strides[2] = {(uint64_t)3 * inner * 2, (uint64_t)seq * 3 * inner * 2};
+  const uint32_t box[3] = {64, 128, 1};
+  int rc = encode_tmap_f16(&pl->tm, qkv, 3, dims, strides, box);
   if (rc) return rc;
   pl->p.seq = seq;
   pl->p.heads = heads;

@@ -78,6 +78,14 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
+                                            int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
+          "r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 
 // Programmatic dependent launch: a kernel launched with the PDL attribute may start while its predecessor is still
 // draining; everything before pdl_wait() (smem carve-up, barrier init, descriptor prefetch) overlaps the predecessor's

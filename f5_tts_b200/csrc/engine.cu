@@ -184,10 +184,6 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
               arch->dim, arch->ff_inner);
     return -1;
   }
-  if (arch->dim / 16 != 64) {
-    set_error("engine_create: ConvPositionEmbedding(groups=16) is built for 64 channels per group, i.e. dim == 1024");
-    return -1;
-  }
   if (arch->conv_layers > 8 || (arch->conv_layers > 0 && (arch->text_dim % 64 || arch->text_dim > 512))) {
     set_error("engine_create: text conv blocks need text_dim %% 64 == 0, <= 512, at most 8 layers");
     return -1;
@@ -305,6 +301,7 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
     a.rows = L.N;
     a.batches = L.Be;
     a.n_out = D;
+    a.k = D / 16;  // ConvPositionEmbedding(groups=16): channels per group
     a.lda = D;
     a.conv_taps = 31;
     a.act = F5_ACT_MISH;

@@ -46,28 +46,35 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-int encode_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
-                    uint64_t stride2, uint32_t b0, uint32_t b1, int rank) {
+int encode_tmap_f16(CUtensorMap* m, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides,
+                    const uint32_t* box) {
   EncodeTiledFn fn = get_encode_fn();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled unavailable (no CUDA driver / not a TMA-capable device)");
     return -3;
   }
-  if ((reinterpret_cast<uintptr_t>(ptr) & 15) || (stride1 & 15) || (rank == 3 && (stride2 & 15))) {
-    set_error("tensor map: pointer/strides must be 16-byte aligned (ptr=%p s1=%llu s2=%llu)", ptr,
-              (unsigned long long)stride1, (unsigned long long)stride2);
+  bool aligned = !(reinterpret_cast<uintptr_t>(ptr) & 15);
+  for (int i = 0; i + 1 < rank; ++i) aligned = aligned && !(strides[i] & 15);
+  if (!aligned) {
+    set_error("tensor map: pointer/strides must be 16-byte aligned (ptr=%p s1=%llu)", ptr,
+              (unsigned long long)strides[0]);
     return -4;
   }
-  cuuint64_t dims[3] = {d0, d1, d2};
-  cuuint64_t strides[2] = {stride1, stride2};
-  cuuint32_t box[3] = {b0, b1, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  cuuint64_t gd[4];
+  cuuint64_t gs[3];
+  cuuint32_t bx[4];
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  for (int i = 0; i < rank; ++i) {
+    gd[i] = dims[i];
+    bx[i] = box[i];
+    if (i + 1 < rank) gs[i] = strides[i];
+  }
+  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), gd, gs, bx, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed: %d (dims %llu,%llu,%llu box %u,%u)", (int)r, (unsigned long long)d0,
-              (unsigned long long)d1, (unsigned long long)d2, b0, b1);
+    set_error("cuTensorMapEncodeTiled failed: %d (rank %d dims %llu,%llu box %u,%u)", (int)r, rank,
+              (unsigned long long)dims[0], (unsigned long long)dims[1], box[0], box[1]);
     return -5;
   }
   return 0;
@@ -280,29 +287,40 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 #endif
   int rc;
   if (conv) {
-    if (a->n_out % 64 || a->lda < a->n_out) {
-      set_error("conv gemm: channels must be a multiple of 64 (got %d, lda %d)", a->n_out, a->lda);
+    const int G = a->k == 0 ? 64 : a->k;  // channels per group
+    if (G <= 0 || G % 8 || G > 64 || a->n_out % G || a->lda < a->n_out) {
+      set_error("conv gemm: channels per group must be a multiple of 8, at most 64, and divide the channel count "
+                "(got %d per group, %d channels, lda %d)", G, a->n_out, a->lda);
       return -1;
     }
     p.num_kb = a->conv_taps;
-    // activations [batches][rows][lda]: channel slice of 64 = one group
-    rc = encode_tmap_f16(&pl->tmA, A, (uint64_t)a->lda, (uint64_t)a->rows, (uint64_t)a->batches, (uint64_t)a->lda * 2,
-                         (uint64_t)a->rows * a->lda * 2, 64, 128, 3);
-    if (rc) return rc;
-    rc = encode_tmap_f16(&pl->tmB, W, 64, (uint64_t)a->conv_taps * a->n_out, 1, 128, 0, 64, 64, 2);
-    if (rc) return rc;
+    p.conv_g = G;
+    // activations [batches][rows][lda] viewed as {G, groups, rows, batches}: a 64-wide box at group g holds the G
+    // channels of g and zeros past them, so a group never reads another group's channels
+    const uint64_t dA[4] = {(uint64_t)G, (uint64_t)(a->n_out / G), (uint64_t)a->rows, (uint64_t)a->batches};
+    const uint64_t sA[3] = {(uint64_t)G * 2, (uint64_t)a->lda * 2, (uint64_t)a->rows * a->lda * 2};
+    const uint32_t bA[4] = {64, 1, 128, 1};
+    if ((rc = encode_tmap_f16(&pl->tmA, A, 4, dA, sA, bA))) return rc;
+    // weights [taps][n_out][G]: input columns past G are zero-filled; box rows past the group's G output channels
+    // only feed accumulator columns that are never stored
+    const uint64_t dW[2] = {(uint64_t)G, (uint64_t)a->conv_taps * a->n_out};
+    const uint64_t sW[1] = {(uint64_t)G * 2};
+    const uint32_t bW[2] = {64, 64};
+    if ((rc = encode_tmap_f16(&pl->tmB, W, 2, dW, sW, bW))) return rc;
   } else {
     if (a->k <= 0 || a->lda < a->k || a->ldw < a->k) {
       set_error("gemm: bad k/lda/ldw (%d, %d, %d)", a->k, a->lda, a->ldw);
       return -1;
     }
     p.num_kb = (a->k + kBK - 1) / kBK;
-    rc = encode_tmap_f16(&pl->tmA, A, (uint64_t)a->k, (uint64_t)a->rows, (uint64_t)a->batches, (uint64_t)a->lda * 2,
-                         (uint64_t)a->rows * a->lda * 2, 64, 128, 3);
-    if (rc) return rc;
-    rc = encode_tmap_f16(&pl->tmB, W, (uint64_t)a->k, (uint64_t)a->n_out, 1, (uint64_t)a->ldw * 2, 0, 64, (uint32_t)bn,
-                         2);
-    if (rc) return rc;
+    const uint64_t dA[3] = {(uint64_t)a->k, (uint64_t)a->rows, (uint64_t)a->batches};
+    const uint64_t sA[2] = {(uint64_t)a->lda * 2, (uint64_t)a->rows * a->lda * 2};
+    const uint32_t bA[3] = {64, 128, 1};
+    if ((rc = encode_tmap_f16(&pl->tmA, A, 3, dA, sA, bA))) return rc;
+    const uint64_t dW[2] = {(uint64_t)a->k, (uint64_t)a->n_out};
+    const uint64_t sW[1] = {(uint64_t)a->ldw * 2};
+    const uint32_t bW[2] = {64, (uint32_t)bn};
+    if ((rc = encode_tmap_f16(&pl->tmB, W, 2, dW, sW, bW))) return rc;
   }
   if (a->epi == F5_EPI_RESID && (a->ldo % 4 || a->resid == nullptr)) {
     set_error("gemm: RESID epilogue needs resid != NULL and ldo %% 4 == 0 (ldo=%d)", a->ldo);
@@ -312,7 +330,8 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     set_error("gemm: fp16 epilogue needs out != NULL and ldo %% 8 == 0 (ldo=%d)", a->ldo);
     return -1;
   }
-  const long long tiles = (long long)((a->n_out + bn - 1) / bn) * ((a->rows + kBM - 1) / kBM) * a->batches;
+  const long long tiles_n = conv ? a->n_out / p.conv_g : (a->n_out + bn - 1) / bn;
+  const long long tiles = tiles_n * ((a->rows + kBM - 1) / kBM) * a->batches;
   pl->grid = dim3((unsigned)(tiles < num_sms() ? tiles : num_sms()), 1, 1);  // persistent: one CTA per SM
   return 0;
 }
@@ -321,7 +340,7 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 
 extern "C" {
 
-int f5_version(void) { return 102; }
+int f5_version(void) { return 103; }
 const char* f5_last_error(void) { return f5::g_err; }
 unsigned long long f5_launch_count(void) { return f5::g_launches.load(); }
 

@@ -12,10 +12,13 @@
 // Pipeline: smem full / empty mbarriers (TMA <-> wgmma); every consumer warp releases a slot once its MMAs retired.
 // Tails in M, N and K come from TMA out-of-bounds zero fill plus guarded stores.
 //
-// CONV mode computes the reference's grouped Conv1d(k=31, groups=16, padding=15) (model/modules.py:175-201)
-// as 31 accumulated 128x64x64 GEMMs: tap t multiplies the activation tile shifted by (t - 15) rows — the shift is
-// just the TMA row coordinate, and rows outside [0, seq) of the SAME sample are zero-filled by the 3-D tensor map,
-// which is exactly the conv's zero padding.
+// CONV mode computes the reference's grouped Conv1d(k=31, groups=16, padding=15) (model/modules.py:175-201) with
+// G = conv_g channels per group (a multiple of 8, at most 64; G = dim / 16) as 31 accumulated 128x64x64 GEMMs per
+// (row tile, group): tap t multiplies the activation tile shifted by (t - 15) rows — the shift is just the TMA row
+// coordinate, and rows outside [0, seq) of the SAME sample are zero-filled by the 4-D tensor map {G, groups, rows,
+// batches}, which is exactly the conv's zero padding.  Columns G..63 of the A and W tiles are zero-filled too, so a
+// group never reads its neighbours' channels; at G < 64 the tensor cores do 64 / G times the algorithmic work.
+// Output columns n0 + G.. of a tile are never stored.
 #pragma once
 #include "common.cuh"
 #include "kparams.h"
@@ -56,13 +59,16 @@ __device__ __forceinline__ bool tile_is_padding(const GemmParams& p, int m0, int
 }
 
 // Fused epilogue of one thread's accumulator fragment: rows row0 and row0 + 8 (half h = 0, 1), columns
-// n0 + 8 j + c2 (+ 1) in acc[4 j + 2 h] (+ 1).  It runs over chunks of 8 to 64 columns, and every global load of a
-// chunk (bias, gate, RoPE cos / sin, residual) is issued before the first store of the chunk.  Stores may alias those
-// inputs as far as the compiler knows, so a loop that loads and stores per column pair waits one full memory latency
-// per pair; here a chunk waits about once.
-template <int BN, int EPI, int ACT>
+// n0 + 8 j + c2 (+ 1) in acc[4 j + 2 h] (+ 1), up to n_end().  It runs over chunks of 8 to 64 columns, and every global
+// load of a chunk (bias, gate, RoPE cos / sin, residual) is issued before the first store of the chunk.  Stores may
+// alias those inputs as far as the compiler knows, so a loop that loads and stores per column pair waits one full
+// memory latency per pair; here a chunk waits about once.
+template <int BN, int EPI, int ACT, bool CONV>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* acc, int n0, int c2, int row0, int bz,
                                               const float* gate) {
+  // first column not stored: a CONV tile ends with its group.  Evaluated at each use, so the plain kernels compile
+  // exactly as when they compared with p.n_out directly.
+  auto n_end = [&]() { return CONV ? n0 + p.conv_g : p.n_out; };
   // chunk width: the widest whose loads fit beside the BN / 2 accumulators without spilling (ptxas caps a 288-thread
   // CTA at 168 registers per thread)
   constexpr int CW = BN <= 128 ? (EPI == EPI_QKV_ROPE ? 32 : 64)
@@ -89,7 +95,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
 #pragma unroll
   for (int cc = 0; cc < BN / CW; ++cc) {
     const int nb = n0 + CW * cc;
-    if (nb >= p.n_out) break;
+    if (nb >= n_end()) break;
     // ---- loads ----
     float2 b[J], g[J];
 #pragma unroll
@@ -97,8 +103,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
       const int nc = nb + 8 * j + c2;
       b[j] = make_float2(0.0f, 0.0f);
       g[j] = make_float2(1.0f, 1.0f);
-      if (nc >= p.n_out) continue;
-      const bool pair_ok = nc + 1 < p.n_out;
+      if (nc >= n_end()) continue;
+      const bool pair_ok = nc + 1 < n_end();
       if (p.bias != nullptr) {
         if (pair_ok) b[j] = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
         else b[j].x = __ldg(p.bias + nc);
@@ -133,8 +139,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           const int nc = nb + 8 * j + c2;
           const float* o = p.resid + grow[h] * p.ldo + nc;
           x[h][j] = make_float2(0.0f, 0.0f);
-          if (!in[h] || nc >= p.n_out) continue;
-          if (nc + 1 < p.n_out) x[h][j] = *reinterpret_cast<const float2*>(o);  // ldo % 4 == 0, nc even: aligned
+          if (!in[h] || nc >= n_end()) continue;
+          if (nc + 1 < n_end()) x[h][j] = *reinterpret_cast<const float2*>(o);  // ldo % 4 == 0, nc even: aligned
           else x[h][j].x = o[0];
         }
     }
@@ -145,8 +151,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
 #pragma unroll
       for (int j = 0; j < J; ++j) {
         const int nc = nb + 8 * j + c2;
-        if (nc >= p.n_out) continue;
-        const bool pair_ok = nc + 1 < p.n_out;
+        if (nc >= n_end()) continue;
+        const bool pair_ok = nc + 1 < n_end();
         float v0 = acc[4 * (J * cc + j) + 2 * h], v1 = acc[4 * (J * cc + j) + 2 * h + 1];
         if (p.bias != nullptr) {
           v0 += b[j].x;
@@ -226,7 +232,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int warp = threadIdx.x >> 5;
   const int cta_id = int(blockIdx.x);
   const int cta_step = int(gridDim.x);
-  const int tiles_n = (p.n_out + BN - 1) / BN;
+  // CONV: one output tile per group of conv_g channels; the tile's columns past conv_g are computed, never stored
+  const int tile_w = CONV ? p.conv_g : BN;
+  const int tiles_n = CONV ? p.n_out / p.conv_g : (p.n_out + BN - 1) / BN;
   const int tiles_m = (p.rows + kBM - 1) / kBM;
   const int num_tiles = tiles_n * tiles_m * p.batches;
 
@@ -251,7 +259,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // ===== TMA producer =====
       uint32_t it = 0;  // running k-block counter across tiles -> stage / phase
       auto load_w = [&](int s, int kb, int n0) {
-        if (CONV) tma_load_2d(sB + s * B_BYTES, &tmB, &full[s], 0, kb * p.n_out + n0);  // [tap][out_channel][in 64]
+        if (CONV) tma_load_2d(sB + s * B_BYTES, &tmB, &full[s], 0, kb * p.n_out + n0);  // [tap][out_channel][in G]
         else tma_load_2d(sB + s * B_BYTES, &tmB, &full[s], kb * kBK, n0);
       };
       // weights of the first tile's first k-blocks: in flight before the dependency wait (slots are free at start)
@@ -260,12 +268,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         pre = uint32_t(p.num_kb < STAGES ? p.num_kb : STAGES);
         for (uint32_t kb = 0; kb < pre; ++kb) {
           mbar_expect_tx(&full[kb], A_BYTES + B_BYTES);
-          load_w(int(kb), int(kb), (cta_id % tiles_n) * BN);
+          load_w(int(kb), int(kb), (cta_id % tiles_n) * tile_w);
         }
       }
       pdl_wait();
       for (int t = cta_id; t < num_tiles; t += cta_step) {
-        const int n0 = (t % tiles_n) * BN;
+        const int n0 = (t % tiles_n) * tile_w;
         const int m0 = ((t / tiles_n) % tiles_m) * kBM;
         const int bz = t / (tiles_n * tiles_m);
         if (tile_is_padding<CONV>(p, m0, bz)) continue;
@@ -277,7 +285,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             mbar_expect_tx(&full[s], A_BYTES + B_BYTES);
             load_w(s, kb, n0);
           }
-          if (CONV) tma_load_3d(sA + s * A_BYTES, &tmA, &full[s], n0, m0 + kb - p.conv_pad, bz);  // tap shift
+          if (CONV) tma_load_4d(sA + s * A_BYTES, &tmA, &full[s], 0, t % tiles_n, m0 + kb - p.conv_pad, bz);  // tap shift
           else tma_load_3d(sA + s * A_BYTES, &tmA, &full[s], kb * kBK, m0, bz);
         }
       }
@@ -297,7 +305,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (lane == 0) mbar_arrive(&empty[s]);
     };
     for (int t = cta_id; t < num_tiles; t += cta_step) {
-      const int n0 = (t % tiles_n) * BN;
+      const int n0 = (t % tiles_n) * tile_w;
       const int m0 = ((t / tiles_n) % tiles_m) * kBM;
       const int bz = t / (tiles_n * tiles_m);
       if (tile_is_padding<CONV>(p, m0, bz)) continue;
@@ -323,7 +331,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #ifdef F5_TRACE
       if (p.diag_no_epi) continue;  // main loop alone (F5_GEMM_EPI=none)
 #endif
-      epilogue_tile<BN, EPI, ACT>(p, acc, n0, c2, m0 + r_in_tile, bz, gate);
+      epilogue_tile<BN, EPI, ACT, CONV>(p, acc, n0, c2, m0 + r_in_tile, bz, gate);
     }
   }
 }

@@ -53,9 +53,10 @@ int attn_plan(AttnPlan* plan, const void* qkv, void* out, int batches, int seq, 
               float scale);
 int attn_run(const AttnPlan& plan, cudaStream_t s);
 
-// 3-D fp16 tensor map: dims (d0 contiguous, d1, d2), byte strides for d1, d2, box (b0, b1, 1), 128B swizzle
-int encode_tmap_f16(CUtensorMap* m, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
-                    uint64_t stride2, uint32_t b0, uint32_t b1, int rank);
+// fp16 tensor map of rank 2 to 4, 128B swizzle: dims[0] is contiguous, strides[i] is the byte stride of dims[i + 1],
+// box[i] the box extent along dims[i].  Box elements outside the tensor are zero-filled by TMA.
+int encode_tmap_f16(CUtensorMap* m, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides,
+                    const uint32_t* box);
 
 }  // namespace f5
 

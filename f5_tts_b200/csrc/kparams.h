@@ -36,6 +36,7 @@ struct GemmParams {
   int conv_pad;  // CONV: taps/2
   int skip_pad;    // 1: 128-row tiles whose rows all lie past their sample's row_len are not computed
   int w_prefetch;  // W tiles may be loaded before griddepcontrol.wait (weights are not produced by the predecessor)
+  int conv_g;      // CONV: channels per group (<= 64); one output tile computes one group
 #ifdef F5_TRACE
   int diag_no_epi;  // instrumented build: skip the epilogue (nothing is stored) to time the main loop alone
 #endif

@@ -79,12 +79,14 @@ def gemm_tile(M: int, N: int, K: int, epi=EPI_F16, act=ACT_NONE, bn=0, pair=0):
 
 
 def grouped_conv31(x: torch.Tensor, w_packed: torch.Tensor, bias, *, resid=None, row_len=None):
-    """Conv1d(k=31, groups=D/64, pad=15) + bias + (mask) + Mish over x fp16 [B, N, D]; w_packed fp16 [31, D, 64].
+    """Conv1d(k=31, groups=D/G, pad=15) + bias + (mask) + Mish over x fp16 [B, N, D]; w_packed fp16 [31, D, G] with
+    G = w_packed.shape[2] channels per group (a multiple of 8, at most 64, dividing D; the model's is D/16).
     resid given: resid += result (fp32, in place) else returns fp16 [B, N, D]."""
     _need_cuda(x, w_packed, bias)
     B, N, D = x.shape
     g = _lib.GemmArgs()
     g.rows, g.batches, g.n_out, g.lda, g.conv_taps, g.act = N, B, D, D, 31, ACT_MISH
+    g.k = w_packed.shape[2]
     g.bias = _ptr(bias)
     g.ldo, g.seq, g.row_len = D, N, _ptr(row_len)
     g.weights_static = 1

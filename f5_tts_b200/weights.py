@@ -5,7 +5,8 @@
    [depth*6D + 2D, D] matrix (rows per block in the reference's chunk order shift_msa, scale_msa, gate_msa,
    shift_mlp, scale_mlp, gate_mlp — model/modules.py:323; final: scale, shift — modules.py:344);
  * input_embed.proj K padded with zero columns to a multiple of 64;
- * grouped Conv1d(k=31, g=16) weight [D, 64, 31] -> [31][D][64] so that tap t / group g is a K-major 64x64 tile;
+ * grouped Conv1d(k=31, g=16) weight [D, G, 31] -> [31][D][G], G = D/16 channels per group, so that tap t / group g
+   is a K-major G x G block (64 x 64 at D = 1024);
  * biases, norm gains, GRN parameters, embedding table -> fp32.
 The packed tensors are owned by Python (kept alive in the returned dict); the C engine only stores pointers.
 """
@@ -53,8 +54,8 @@ def packed_tensors(m) -> dict[str, torch.Tensor]:
     pwp[:, :kin] = pw.to(torch.float16)
     T["proj_w"], T["proj_b"] = pwp, _f(sd["input_embed.proj.bias"])
     for j, idx in enumerate((0, 2)):
-        cw = sd[f"input_embed.conv_pos_embed.conv1d.{idx}.weight"]  # [D_out, 64, 31]
-        T[f"conv_w{j}"] = _h(cw.permute(2, 0, 1))                     # [31, D_out, 64]
+        cw = sd[f"input_embed.conv_pos_embed.conv1d.{idx}.weight"]  # [D_out, G, 31]
+        T[f"conv_w{j}"] = _h(cw.permute(2, 0, 1))                     # [31, D_out, G]
         T[f"conv_b{j}"] = _f(sd[f"input_embed.conv_pos_embed.conv1d.{idx}.bias"])
     for i in range(depth):
         q = f"L{i}."

@@ -39,14 +39,15 @@ enum { F5_ACT_NONE = 0, F5_ACT_GELU_TANH = 1, F5_ACT_GELU_ERF = 2, F5_ACT_MISH =
 enum { F5_EPI_F16 = 0, F5_EPI_F32 = 1, F5_EPI_RESID = 2, F5_EPI_QKV_ROPE = 3 };
 
 /* Fused linear: C = epilogue(A[M,K] . W[N,K]^T) — replaces nn.Linear (aten::addmm) call sites
- * model/modules.py:317,338,360-361,398-400 and, with conv != 0, the grouped Conv1d(k=taps, groups=D/64,
- * padding=taps/2) of ConvPositionEmbedding (model/modules.py:175-201).
- *   A fp16 [batches*rows, lda]; W fp16 [N, ldw] (conv: [taps][N][64]); fp32 accumulation. */
+ * model/modules.py:317,338,360-361,398-400 and, with conv_taps != 0, the grouped Conv1d(k=taps, groups=N/k,
+ * padding=taps/2) of ConvPositionEmbedding (model/modules.py:175-201), k channels per group.
+ *   A fp16 [batches*rows, lda]; W fp16 [N, ldw] (conv: [taps][N][k]); fp32 accumulation. */
 typedef struct {
   int rows;      /* valid rows per batch entry (plain GEMM: M, batches = 1) */
   int batches;
   int n_out;
-  int k;         /* reduction length (plain) ; ignored for conv */
+  int k;         /* reduction length (plain) ; conv: channels per group, 0 = 64 (a multiple of 8, <= 64, dividing
+                    n_out; anything else is rejected) */
   int lda, ldw;  /* elements */
   int bn;        /* output tile width: 64 | 128 | 192 | 256 (0 = the planner picks the width) */
   int epi, act;
@@ -144,7 +145,7 @@ typedef struct {
   } text_blocks[8];
   const void* proj_w; const float* proj_b;    /* fp16 [D, Kpad] input_embed.proj, K zero-padded to a multiple of 64 */
   int proj_kpad;
-  const void* conv_w[2]; const float* conv_b[2]; /* fp16 [31][D][64] re-packed grouped conv, fp32 [D] */
+  const void* conv_w[2]; const float* conv_b[2]; /* fp16 [31][D][D/16] re-packed grouped conv, fp32 [D] */
   const void* mod_w; const float* mod_b;      /* DiT: fp16 [depth*6D + 2D, D] all AdaLN linears stacked; fp32 bias */
   const f5_layer_weights* layers;             /* [depth] */
   const float* g_out;                         /* UNetT norm_out.g */

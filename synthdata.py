@@ -52,6 +52,19 @@ def e2tts_base() -> ArchConfig:  # configs/E2TTS_Base.yaml:25-31
                       text_mask_padding=False, pe_attn_head=1)
 
 
+def f5tts_small() -> ArchConfig:  # configs/F5TTS_Small.yaml:25-35
+    return ArchConfig(dim=768, depth=18, heads=12)
+
+
+def f5tts_v1_small() -> ArchConfig:  # configs/F5TTS_v1_Small.yaml:26-36
+    return ArchConfig(dim=768, depth=18, heads=12, text_mask_padding=True, pe_attn_head=None)
+
+
+def e2tts_small() -> ArchConfig:  # configs/E2TTS_Small.yaml:25-31
+    return ArchConfig(backbone="UNetT", dim=768, depth=20, heads=12, ff_mult=4, text_dim=None, conv_layers=0,
+                      text_mask_padding=False, pe_attn_head=1)
+
+
 # ---------------------------------------------------------------------------
 # synthetic weights in the released checkpoint layout
 # ---------------------------------------------------------------------------

@@ -3,6 +3,8 @@
 Every row ends with the same shape through cuBLAS (torch.matmul fp16, no epilogue) as a comparator.
 SWEEP_M=<M,...> picks the row counts; SWEEP_TILES=auto times only the planner's pick.  With the instrumented library
 (F5_LIB=f5_tts_b200/libf5tts_b200_trace.so) and F5_GEMM_EPI=none the times are of the main loop alone.
+SWEEP_CONV=1 instead times the conv position embedding pair (Conv1d(k=31, groups=16) + Mish to fp16, then the same
+with the fp32 residual add) at B = 2, N = 938 for dim 768 (48 channels per group) and dim 1024 (64 per group).
 """
 import os
 import sys
@@ -39,6 +41,27 @@ def cublas(M, N, K, nw):
     wt = [(torch.randn(N, K, generator=g) / 32).half().to(DEV).t() for _ in range(nw)]
     return _graph_time_us(lambda: [torch.matmul(a[i % 2], wt[i]) for i in range(nw)], nw, rounds=4)
 
+
+def conv_pair(D, B=2, N=938, nw=8):
+    G = D // 16
+    x = torch.randn(B, N, D, generator=g).half().to(DEV)
+    w = [(torch.randn(31, D, G, generator=g) / (G * 31) ** 0.5).half().to(DEV) for _ in range(2 * nw)]
+    b = torch.randn(D, generator=g).to(DEV)
+    r = torch.zeros(B, N, D, device=DEV)
+
+    def pair(i):
+        c = ops.grouped_conv31(x, w[2 * i], b)
+        ops.grouped_conv31(c, w[2 * i + 1], b, resid=r)
+
+    us = _graph_time_us(lambda: [pair(i) for i in range(nw)], nw, rounds=20)
+    return us, 2 * 2.0 * B * N * D * G * 31 / (us * 1e-6) / 1e12
+
+
+if os.environ.get("SWEEP_CONV"):
+    for D in (768, 1024):
+        us, tf = conv_pair(D)
+        print(f"conv pair D={D} G={D // 16} B=2 N=938: {us:6.1f}us per pair  {tf:5.1f} algorithmic TF", flush=True)
+    sys.exit(0)
 
 Ms = [int(x) for x in os.environ.get("SWEEP_M", "1876,3752,7504,15008").split(",")]
 pick_only = os.environ.get("SWEEP_TILES", "all") == "auto"

@@ -3,7 +3,9 @@ F5_DIAG_SKIP=<kernel class> to read the in-situ cost of that class as the differ
 
 STEP_ODE=<method>:<steps>[,<method>:<steps>...] times each ODE solver setting in turn (default euler:<workload NFE>),
 STEP_ROUNDS=<n> repeats the whole list n times, alternating, so that settings are compared within one process
-(e.g. STEP_ODE=euler:32,midpoint:16 — both make 32 backbone evaluations)."""
+(e.g. STEP_ODE=euler:32,midpoint:16 — both make 32 backbone evaluations).
+STEP_ARCH=<preset>[,<preset>...] (synthdata presets, default the workload's arch) times each architecture on the same
+inputs, alternating within every round (e.g. STEP_ARCH=f5tts_v1_base,f5tts_v1_small)."""
 import os
 import subprocess
 import sys
@@ -18,7 +20,10 @@ name = os.environ.get("STEP_WORKLOAD", "cfg2")
 w = bench.WORKLOADS[name]
 runs = [(m, int(s)) for m, s in (p.split(":") for p in os.environ.get("STEP_ODE", f"euler:{w['nfe']}").split(","))]
 rounds = int(os.environ.get("STEP_ROUNDS", "1"))
-model, voc, _ = bench.build_gpu_model(w["arch"], dev)
+archs = os.environ.get("STEP_ARCH", w["arch"]).split(",")
+models = {}
+for a in archs:
+    models[a], voc, _ = bench.build_gpu_model(a, dev)
 wav, text, duration, lens = (t.to(dev) for t in bench.synth_inputs(w))
 try:
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
@@ -28,7 +33,7 @@ except (OSError, subprocess.SubprocessError):
 print(f"device: {card}")
 
 
-def time_call(method, steps, n=5):
+def time_call(model, method, steps, n=5):
     model.odeint_kwargs = dict(method=method)
     fn = lambda: bench.hot_path(model, voc, wav, text, duration, lens, steps)  # noqa: E731
     for _ in range(3):
@@ -44,8 +49,9 @@ def time_call(method, steps, n=5):
 
 
 for r in range(rounds):
-    for method, steps in runs:
-        nfe = 2 * steps if method == "midpoint" else steps
-        ms = time_call(method, steps)
-        print(f"{name} ode={method} steps={steps} nfe={nfe} round={r} ms_per_call {ms:.3f}  "
-              f"per_NFE_us {ms * 1e3 / nfe:.1f}  skip={os.environ.get('F5_DIAG_SKIP', '')}")
+    for arch in archs:
+        for method, steps in runs:
+            nfe = 2 * steps if method == "midpoint" else steps
+            ms = time_call(models[arch], method, steps)
+            print(f"{name} arch={arch} ode={method} steps={steps} nfe={nfe} round={r} ms_per_call {ms:.3f}  "
+                  f"per_NFE_us {ms * 1e3 / nfe:.1f}  skip={os.environ.get('F5_DIAG_SKIP', '')}")
