@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("F5_LIB") or os.path.join(_HERE, "libf5tts_b200.so")  
 c_void_p, c_int, c_float, c_size_t, c_ll = C.c_void_p, C.c_int, C.c_float, C.c_size_t, C.c_longlong
 
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_ERF, ACT_MISH = 0, 1, 2, 3
-EPI_F16, EPI_F32, EPI_RESID, EPI_QKV_ROPE = 0, 1, 2, 3
+EPI_F16, EPI_F32, EPI_RESID, EPI_QKV_ROPE, EPI_QKV_NORM_ROPE = 0, 1, 2, 3, 4
 
 
 class GemmArgs(C.Structure):
@@ -27,7 +27,7 @@ class GemmArgs(C.Structure):
         ("gate", c_void_p), ("step_ptr", c_void_p), ("gate_step_stride", c_ll), ("row_len", c_void_p),
         ("seq", c_int), ("rope_cos", c_void_p), ("rope_sin", c_void_p), ("inner", c_int), ("pe_heads", c_int),
         ("weights_static", c_int),
-        ("skip_padded_tiles", c_int),
+        ("skip_padded_tiles", c_int), ("q_norm", c_void_p), ("k_norm", c_void_p),
     ]
 
 
@@ -44,12 +44,12 @@ class VocosWeights(C.Structure):
 class Arch(C.Structure):
     _fields_ = [(n, c_int) for n in ("backbone", "dim", "depth", "heads", "dim_head", "ff_inner", "mel_dim", "text_dim",
                                      "text_num_embeds", "conv_layers", "text_mask_padding", "pe_attn_head",
-                                     "attn_mask_enabled")]
+                                     "attn_mask_enabled", "qk_norm", "long_skip", "text_avg_upsample")]
 
 
 class LayerWeights(C.Structure):
     _fields_ = [(n, c_void_p) for n in ("w_qkv", "b_qkv", "w_out", "b_out", "w_ff1", "b_ff1", "w_ff2", "b_ff2",
-                                        "w_skip", "g_attn", "g_ff")]
+                                        "w_skip", "g_attn", "g_ff", "q_norm_w", "k_norm_w")]
 
 
 class TextBlock(C.Structure):
@@ -65,6 +65,7 @@ class Weights(C.Structure):
         ("conv_w", c_void_p * 2), ("conv_b", c_void_p * 2),
         ("mod_w", c_void_p), ("mod_b", c_void_p),
         ("layers", C.POINTER(LayerWeights)), ("g_out", c_void_p), ("out_w", c_void_p), ("out_b", c_void_p),
+        ("long_skip_w", c_void_p),
     ]
 
 

@@ -169,6 +169,53 @@ __global__ void text_gather_kernel(const TextGatherParams p) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// text_embedding_average_upsampling (backbones/dit.py:55-84, 131-137): sample b's T valid text rows (filler == 0, the
+// cond variant's mask for both variants) are spread over its A audio rows, token j repeated A / T times plus once
+// more for the last A % T tokens; rows at or past A, and every row when T == 0, are 0.  A = valid_len[b], or N.
+// grid (B, ceil(N / rows_per_block)); each block compacts the first K = min(nt, N) filler flags of its sample into
+// shared memory (positions at or past nt are always filler), then writes rows of both variants.
+// tx, out fp32 [2B, N, Td]; filler [B, N]; dynamic smem K ints.
+// ---------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) text_avg_upsample_kernel(const float* tx, float* out, const uint8_t* filler,
+                                                                const int* valid_len, int B, int N, int K, int Td,
+                                                                int rows_per_block) {
+  extern __shared__ int vidx[];  // [K] positions of the valid text rows, in order
+  __shared__ int warp_cnt[8];
+  const int b = blockIdx.x;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  int T = 0;
+  for (int t0 = 0; t0 < K; t0 += 256) {
+    const int k = t0 + threadIdx.x;
+    const bool v = k < K && filler[(long long)b * N + k] == 0;
+    const unsigned m = __ballot_sync(0xffffffffu, v);
+    if (lane == 0) warp_cnt[w] = __popc(m);
+    __syncthreads();
+    int off = T;
+    for (int i = 0; i < w; ++i) off += warp_cnt[i];
+    if (v) vidx[off + __popc(m & ((1u << lane) - 1u))] = k;
+    for (int i = 0; i < 8; ++i) T += warp_cnt[i];
+    __syncthreads();
+  }
+  const int A = valid_len != nullptr ? min(valid_len[b], N) : N;
+  const int p0 = blockIdx.y * rows_per_block, p1 = min(p0 + rows_per_block, N);
+  for (int p = p0; p < p1; ++p) {
+    int src = -1;
+    if (p < A && T > 0) {
+      const int base = A / T, rem = A % T;
+      const int lead = (T - rem) * base;  // rows of the tokens repeated `base` times (0 when base == 0)
+      const int j = p < lead ? p / base : (T - rem) + (p - lead) / (base + 1);
+      src = vidx[j];
+    }
+    for (int var = 0; var < 2; ++var) {
+      const long long r = (long long)var * B + b;
+      float* o = out + (r * N + p) * Td;
+      const float* s = tx + (r * N + (src < 0 ? 0 : src)) * Td;
+      for (int c = threadIdx.x; c < Td; c += blockDim.x) o[c] = src < 0 ? 0.f : s[c];
+    }
+  }
+}
+
 // rows where filler[b, n] != 0 are zeroed (text_mask_padding, dit.py:123-127); x fp32 [2B, N, C]
 __global__ void mask_rows_kernel(float* x, const uint8_t* filler, int BN, int rows, int C) {
   const int row = blockIdx.x;

@@ -71,6 +71,8 @@ struct Layout {
   __half* cat;
   __half *a, *qkv, *ao, *g;
   float* v;
+  float* x_embed;  // DiT long_skip_connection: x after the input embedding [M1, D] (cat(...) goes to `cat`), else null
+  float* txu;      // text_embedding_average_upsampling: upsampled text [2B, N, Td], else null
   size_t bytes;
 };
 
@@ -165,6 +167,13 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.ao = bp.take<__half>((size_t)L.M1 * e->inner);
   L.g = bp.take<__half>((size_t)L.M1 * F);
   L.v = bp.take<float>((size_t)L.M1 * A.mel_dim);
+  // buffers of the architecture options last: with the options off the layout is the one above
+  L.x_embed = nullptr;
+  if (A.long_skip) {
+    L.x_embed = bp.take<float>((size_t)L.M1 * D);
+    L.cat = bp.take<__half>((size_t)L.M1 * 2 * D);
+  }
+  L.txu = A.text_avg_upsample ? bp.take<float>((size_t)2 * B * N * Td) : nullptr;
   L.bytes = bp.off + 512;
 }
 
@@ -188,6 +197,24 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
     set_error("engine_create: text conv blocks need text_dim %% 64 == 0, <= 512, at most 8 layers");
     return -1;
   }
+  if ((arch->long_skip || arch->text_avg_upsample) && arch->backbone != 0) {
+    set_error("engine_create: long_skip and text_avg_upsample are DiT options");
+    return -1;
+  }
+  if (arch->text_avg_upsample && !arch->text_mask_padding) {
+    set_error("engine_create: text_avg_upsample needs text_mask_padding (backbones/dit.py:41-43)");
+    return -1;
+  }
+  if (arch->long_skip && weights->long_skip_w == nullptr) {
+    set_error("engine_create: long_skip needs long_skip_w");
+    return -1;
+  }
+  if (arch->qk_norm)
+    for (int i = 0; i < arch->depth; ++i)
+      if (weights->layers[i].q_norm_w == nullptr || weights->layers[i].k_norm_w == nullptr) {
+        set_error("engine_create: qk_norm needs q_norm_w and k_norm_w in every layer (layer %d)", i);
+        return -1;
+      }
   if (int rc = configure_kernels()) return rc;
   f5_engine* e = new f5_engine();
   e->arch = *arch;
@@ -226,6 +253,7 @@ double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_stre
     const double n = N;
     per = Ld * (8.0 * n * D * D + 4.0 * n * D * F + 4.0 * n * n * D) + 2.0 * n * (2 * mel + Td) * D +
           2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n * D * mel;
+    if (A.long_skip) per += 2.0 * n * D * (2.0 * D);  // long_skip_connection: Linear(2D -> D)
   } else {
     const double n1 = N + 1.0, n = N;
     per = Ld * (8.0 * n1 * D * D + 4.0 * n1 * D * F + 4.0 * n1 * n1 * D) + (Ld / 2.0) * 4.0 * n1 * D * D +
@@ -245,7 +273,7 @@ double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_stre
 namespace {
 
 struct StepPlans {
-  GemmPlan proj, conv1, conv2, out_proj;
+  GemmPlan proj, conv1, conv2, out_proj, long_skip;
   std::vector<GemmPlan> qkv, oproj, ff1, ff2, skip;
   std::vector<AttnPlan> attn;  // identical per layer, kept once
 };
@@ -345,7 +373,10 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
       RC(gemm_plan(&P.skip[i], L.cat, lw.w_skip, &a));  // (EPI_F32 direct-store path: not tile-skipped)
     }
     {
-      f5_gemm_args a = base_args(L.M1, 3 * inner, D, D, D, kAutoTile, F5_EPI_QKV_ROPE, F5_ACT_NONE);
+      f5_gemm_args a = base_args(L.M1, 3 * inner, D, D, D, kAutoTile, A.qk_norm ? F5_EPI_QKV_NORM_ROPE : F5_EPI_QKV_ROPE,
+                                 F5_ACT_NONE);
+      a.q_norm = lw.q_norm_w;
+      a.k_norm = lw.k_norm_w;
       a.bias = lw.b_qkv;
       a.out = L.qkv;
       a.ldo = 3 * inner;
@@ -393,6 +424,12 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
       varlen(a);
       RC(gemm_plan(&P.ff2[i], L.g, lw.w_ff2, &a));
     }
+  }
+  if (A.long_skip) {  // x = cat(x, x_embed) . long_skip_w^T, no bias (backbones/dit.py:228, 363-364)
+    f5_gemm_args a = base_args(L.M1, D, 2 * D, 2 * D, 2 * D, 128, F5_EPI_F32, F5_ACT_NONE);
+    a.out = L.x;
+    a.ldo = D;
+    RC(gemm_plan(&P.long_skip, L.cat, W.long_skip_w, &a));
   }
   {
     f5_gemm_args a = base_args(L.M1, A.mel_dim, D, D, D, 128, F5_EPI_F32, F5_ACT_NONE);
@@ -445,6 +482,9 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
     RC(gemm_run(P.conv2, s));
   }
   if (!dit) RC(run_prepend_time_token(L.x, L.h0, L.temb, L.step_ptr, L.N, D, L.M1, s));
+  if (A.long_skip)
+    RC(check_cuda(cudaMemcpyAsync(L.x_embed, L.x, sizeof(float) * L.M1 * D, cudaMemcpyDeviceToDevice, s),
+                  "long skip copy"));
   const int half = A.depth / 2;
   for (int i = 0; i < A.depth; ++i) {
     const f5_layer_weights& lw = e->w.layers[i];
@@ -472,6 +512,10 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
     }
     if (!diag_skip("ff1")) RC(gemm_run(P.ff1[i], s));
     if (!diag_skip("ff2")) RC(gemm_run(P.ff2[i], s));
+  }
+  if (A.long_skip) {
+    RC(run_concat_half(L.x, L.x_embed, L.cat, L.M1, D, s));
+    RC(gemm_run(P.long_skip, s));
   }
   if (dit) {
     const float* m = L.mod + (size_t)A.depth * 6 * D;
@@ -613,6 +657,8 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     if (strict) RC(run_mask_rows_len(L.tx, L.valid_len, B, N, R2, Td, s));
   }
   if (A.conv_layers > 0 && A.text_mask_padding) RC(run_mask_rows(L.tx, L.filler, B * N, R2, Td, s));
+  if (A.text_avg_upsample)  // audio lengths: duration (the reference's seq_len = mask.sum), else N
+    RC(run_text_avg_upsample(L.tx, L.txu, L.filler, masked ? L.valid_len : nullptr, B, N, sa->nt, Td, s));
   PackParams pp{};
   pp.xin = L.xin;
   pp.B = B;
@@ -623,7 +669,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   pp.packed = L.packed;
   pp.y = sa->y;
   pp.step_cond = sa->step_cond;
-  pp.text = L.tx;
+  pp.text = A.text_avg_upsample ? L.txu : L.tx;
   RC(run_pack_input(pp, s));
   if (sa->trajectory)
     RC(check_cuda(cudaMemcpyAsync(sa->trajectory, sa->y, sizeof(float) * B * N * A.mel_dim, cudaMemcpyDeviceToDevice, s),

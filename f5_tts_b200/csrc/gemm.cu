@@ -112,6 +112,9 @@ static const GemmKernel kGemmKernels[] = {
     F5_GEMM_KERNEL(256, EPI_QKV_ROPE, ACT_NONE, false),
     F5_GEMM_KERNEL(64, EPI_F16, ACT_MISH, true),
     F5_GEMM_KERNEL(64, EPI_RESID, ACT_MISH, true),
+    F5_GEMM_KERNEL(128, EPI_QKV_NORM_ROPE, ACT_NONE, false),
+    F5_GEMM_KERNEL(192, EPI_QKV_NORM_ROPE, ACT_NONE, false),
+    F5_GEMM_KERNEL(256, EPI_QKV_NORM_ROPE, ACT_NONE, false),
 };
 #undef F5_GEMM_KERNEL
 
@@ -196,6 +199,8 @@ int gemm_run(const GemmPlan& pl, cudaStream_t s) {
 // Tiles run in rounds over the SMs; the producer streams the next tile's operands during the epilogue, so a round
 // costs main + epilogue.  Checked against the graph-timed sweep of tools/gemm_sweep.py with the chunked epilogue (H100
 // SXM 80 GB, 700 W limit): the pick is the fastest width at M = 1876 and within 11 % of it at M = 3752 - 15008.
+// QKV + RMSNorm + RoPE is costed as QKV + RoPE: its norm pass added 4 % at M = 1876 at every width but 256, where the
+// 128 x 192 pick stays the fastest (tools/qkv_epilogue_time.py, same card).
 // Diagnostic build (make TRACE=1) only: F5_BN_<n_out>=<bn> overrides the choice.
 static int pick_tile(long long rows, int batches, int n_out, int k, int epi, int act) {
 #ifdef F5_TRACE
@@ -253,6 +258,12 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     set_error("gemm: QKV_ROPE needs inner %% 64 == 0, rope tables and seq");
     return -1;
   }
+  if (a->epi == F5_EPI_QKV_NORM_ROPE &&
+      (a->inner <= 0 || a->inner % 64 || a->n_out % 64 || a->rope_cos == nullptr || a->rope_sin == nullptr ||
+       a->seq <= 0 || a->q_norm == nullptr || a->k_norm == nullptr || conv)) {
+    set_error("gemm: QKV_NORM_ROPE needs q_norm and k_norm, inner %% 64 == 0, n_out %% 64 == 0, rope tables and seq");
+    return -1;
+  }
   pl->bn = bn;
   pl->epi = a->epi;
   pl->act = a->act;
@@ -275,6 +286,8 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
   p.rope_sin = a->rope_sin;
   p.inner = a->inner > 0 ? a->inner : 64;
   p.pe_heads = a->pe_heads;
+  p.q_norm = a->q_norm;
+  p.k_norm = a->k_norm;
   p.conv_pad = a->conv_taps / 2;
   p.skip_pad = (a->skip_padded_tiles && a->row_len != nullptr && a->seq > 0 && (conv || a->batches == 1)) ? 1 : 0;
   // a prefetched W tile belongs to the CTA's first tile: not known to be computed when padded tiles are skipped
@@ -326,7 +339,8 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     set_error("gemm: RESID epilogue needs resid != NULL and ldo %% 4 == 0 (ldo=%d)", a->ldo);
     return -1;
   }
-  if ((a->epi == F5_EPI_F16 || a->epi == F5_EPI_QKV_ROPE) && (a->ldo % 8 || a->out == nullptr)) {
+  if ((a->epi == F5_EPI_F16 || a->epi == F5_EPI_QKV_ROPE || a->epi == F5_EPI_QKV_NORM_ROPE) &&
+      (a->ldo % 8 || a->out == nullptr)) {
     set_error("gemm: fp16 epilogue needs out != NULL and ldo %% 8 == 0 (ldo=%d)", a->ldo);
     return -1;
   }
@@ -340,7 +354,7 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 
 extern "C" {
 
-int f5_version(void) { return 104; }
+int f5_version(void) { return 105; }
 const char* f5_last_error(void) { return f5::g_err; }
 unsigned long long f5_launch_count(void) { return f5::g_launches.load(); }
 

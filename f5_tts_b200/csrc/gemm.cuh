@@ -6,7 +6,7 @@
 // together share the A row-panel in L2 and sweep W once).  Warp roles (288 threads):
 //   warps 0..7    two consumer warpgroups: warpgroup g computes rows [64 g, 64 g + 64) of the 128 x BN tile with
 //                 wgmma m64nBNk16 (both operands read from shared memory), then runs the fused bias / activation /
-//                 RoPE / gate / mask epilogue straight from its accumulator registers
+//                 qk RMSNorm / RoPE / gate / mask epilogue straight from its accumulator registers
 //   warp 8        TMA producer (one elected lane): STAGES-deep ring of {A 128x64, W BNx64} fp16 tiles, SWIZZLE_128B.  It
 //                 runs ahead into the next tile's k-blocks while the consumers are in the epilogue.
 // Pipeline: smem full / empty mbarriers (TMA <-> wgmma); every consumer warp releases a slot once its MMAs retired.
@@ -64,15 +64,18 @@ __device__ __forceinline__ bool tile_is_padding(const GemmParams& p, int m0, int
 // alias those inputs as far as the compiler knows, so a loop that loads and stores per column pair waits one full
 // memory latency per pair; here a chunk waits about once.
 template <int BN, int EPI, int ACT, bool CONV>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* acc, int n0, int c2, int row0, int bz,
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, int n0, int c2, int row0, int bz,
                                               const float* gate) {
   // first column not stored: a CONV tile ends with its group.  Evaluated at each use, so the plain kernels compile
   // exactly as when they compared with p.n_out directly.
   auto n_end = [&]() { return CONV ? n0 + p.conv_g : p.n_out; };
+  constexpr bool NORM = EPI == EPI_QKV_NORM_ROPE;
+  constexpr bool QKV = EPI == EPI_QKV_ROPE || NORM;
   // chunk width: the widest whose loads fit beside the BN / 2 accumulators without spilling (ptxas caps a 288-thread
-  // CTA at 168 registers per thread)
-  constexpr int CW = BN <= 128 ? (EPI == EPI_QKV_ROPE ? 32 : 64)
-                     : BN == 192 ? (EPI == EPI_QKV_ROPE ? 16 : 32)
+  // CTA at 168 registers per thread).  QKV_NORM_ROPE adds its bias before the chunks, which frees the bias registers.
+  constexpr int CW = NORM ? (BN <= 128 ? 64 : BN == 192 ? 32 : 8)
+                   : BN <= 128 ? (QKV ? 32 : 64)
+                     : BN == 192 ? (QKV ? 16 : 32)
                                  : (EPI == EPI_F16 ? 32 : EPI == EPI_RESID ? 16 : 8);
   constexpr int J = CW / 8;  // column pairs of one thread in a chunk
   bool in[2], valid[2];
@@ -91,11 +94,43 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
     }
     if (EPI == EPI_RESID) in[h] = in[h] && valid[h];  // masked rows keep their residual
   }
-  if (!in[0] && !in[1]) return;
+  // qk_norm shuffles within quads: every lane of the warp has to reach them, so no lane leaves early
+  if (!NORM && !in[0] && !in[1]) return;
+  float rinv[2];  // qk_norm: 1 / RMS of rows row0, row0 + 8 of the current head
 #pragma unroll
   for (int cc = 0; cc < BN / CW; ++cc) {
     const int nb = n0 + CW * cc;
     if (nb >= n_end()) break;
+    // qk_norm, at the first chunk of a head: the bias goes into the head's accumulators here (the chunks below add none),
+    // then, for a q or k head, 1 / RMS over its 64 columns in fp32.  The head lies in this tile (BN, n0 and CW divide
+    // into 64-column heads); one row of it is spread over the 4 lanes of a quad, 16 values each, so one pass over the
+    // head's registers and two quad shuffles give the sum of squares.  Kept per head, not per tile: 16 live values for a
+    // 256-wide tile spill.
+    if (NORM && ((CW * cc) & 63) == 0) {
+      const int hb = (CW * cc) >> 3;  // first 8-column group of the head
+      const bool qk = nb / p.inner < 2;  // the same for the whole warp
+      float ss[2] = {0.0f, 0.0f};
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float2 b = make_float2(0.0f, 0.0f);
+        if (p.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(p.bias + nb + 8 * j + c2));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float& v0 = acc[4 * (hb + j) + 2 * h];
+          float& v1 = acc[4 * (hb + j) + 2 * h + 1];
+          v0 += b.x;
+          v1 += b.y;
+          if (qk) ss[h] += v0 * v0 + v1 * v1;
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 1);
+        ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 2);
+        rinv[h] = rsqrtf(ss[h] * (1.0f / 64.0f) + 1e-6f);
+      }
+    }
+    if (NORM && !in[0] && !in[1]) continue;
     // ---- loads ----
     float2 b[J], g[J];
 #pragma unroll
@@ -105,7 +140,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
       g[j] = make_float2(1.0f, 1.0f);
       if (nc >= n_end()) continue;
       const bool pair_ok = nc + 1 < n_end();
-      if (p.bias != nullptr) {
+      if (!NORM && p.bias != nullptr) {
         if (pair_ok) b[j] = __ldg(reinterpret_cast<const float2*>(p.bias + nc));
         else b[j].x = __ldg(p.bias + nc);
       }
@@ -114,11 +149,20 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         if (pair_ok) g[j].y = gate[nc + 1];
       }
     }
-    bool rope = false;
+    bool rope = false, nrm = false;
     float rc[2][J], rs[2][J];
-    if (EPI == EPI_QKV_ROPE) {  // inner % 64 == 0 and CW divides 64: a chunk lies in one head of one section
+    float2 gn[J];
+    if (QKV) {  // inner % 64 == 0 and CW divides 64: a chunk lies in one head of one section
       const int sec = nb / p.inner, head = (nb - sec * p.inner) >> 6;
       rope = sec < 2 && head < p.pe_heads;
+      if (NORM) {
+        nrm = sec < 2;
+        if (nrm) {
+          const float* gw = sec == 0 ? p.q_norm : p.k_norm;
+#pragma unroll
+          for (int j = 0; j < J; ++j) gn[j] = __ldg(reinterpret_cast<const float2*>(gw + (nb & 63) + 8 * j + c2));
+        }
+      }
       if (rope) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -154,11 +198,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
         if (nc >= n_end()) continue;
         const bool pair_ok = nc + 1 < n_end();
         float v0 = acc[4 * (J * cc + j) + 2 * h], v1 = acc[4 * (J * cc + j) + 2 * h + 1];
-        if (p.bias != nullptr) {
+        if (!NORM && p.bias != nullptr) {
           v0 += b[j].x;
           if (pair_ok) v1 += b[j].y;
         }
-        if (EPI == EPI_QKV_ROPE && rope) {
+        if (NORM && nrm) {
+          const float r = rinv[h];
+          v0 = v0 * r * gn[j].x;
+          v1 = v1 * r * gn[j].y;
+        }
+        if (QKV && rope) {
           const float c = rc[h][j], s = rs[h][j];
           const float x0 = v0, x1 = v1;
           v0 = x0 * c - x1 * s;
@@ -174,7 +223,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float* 
           v0 = mish(v0);
           v1 = mish(v1);
         }
-        if (EPI == EPI_F16 || EPI == EPI_QKV_ROPE) {
+        if (EPI == EPI_F16 || QKV) {
           __half* o = reinterpret_cast<__half*>(p.out) + grow[h] * p.ldo + nc;
           if (!valid[h]) v0 = v1 = 0.0f;
           if (pair_ok) *reinterpret_cast<uint32_t*>(o) = pack_half2(v0, v1);

@@ -66,6 +66,9 @@ namespace f5 {
 int run_row_norm(int mode, const NormParams& p, cudaStream_t s);
 int run_dwconv7_ln(const DwConvLnParams& p, cudaStream_t s);
 int run_text_gather(const TextGatherParams& p, cudaStream_t s);
+// text_embedding_average_upsampling: tx -> out, both fp32 [2B, N, Td]; valid_len [B] audio lengths or null (= N)
+int run_text_avg_upsample(const float* tx, float* out, const uint8_t* filler, const int* valid_len, int B, int N,
+                          int nt, int Td, cudaStream_t s);
 int run_mask_rows(float* x, const uint8_t* filler, int BN, int rows, int C, cudaStream_t s);
 int run_mask_rows_len(float* x, const int* valid_len, int B, int N, int rows, int C, cudaStream_t s);
 int run_mask_rows_len_half(__half* x, const int* valid_len, int B, int N, int rows, int C, cudaStream_t s);

@@ -12,6 +12,8 @@ enum : int {
   EPI_F32 = 1,       // out32[m,n] = acc + bias ; optional out16b[m,n] = mask(acc + bias) (fp16 copy)
   EPI_RESID = 2,     // resid32[m,n] += gate[n] * mask(act(acc + bias))
   EPI_QKV_ROPE = 3,  // out16[m,n] = rope(acc + bias) for the first pe_heads heads of q,k; plain for the rest
+  // as EPI_QKV_ROPE, with a per-head RMSNorm(64, eps 1e-6, gain q_norm / k_norm) on every q and k head before RoPE
+  EPI_QKV_NORM_ROPE = 4,
 };
 
 struct GemmParams {
@@ -40,6 +42,10 @@ struct GemmParams {
 #ifdef F5_TRACE
   int diag_no_epi;  // instrumented build: skip the epilogue (nothing is stored) to time the main loop alone
 #endif
+  // EPI_QKV_NORM_ROPE: fp32 [64] RMSNorm gains of the q and k heads.  Last, so the other epilogues' kernels keep their
+  // parameter offsets.
+  const float* q_norm;
+  const float* k_norm;
 };
 
 constexpr int kBM = 128;

@@ -83,6 +83,21 @@ int run_text_gather(const TextGatherParams& p, cudaStream_t s) {
   return check_launch("text_gather_kernel");
 }
 
+int run_text_avg_upsample(const float* tx, float* out, const uint8_t* filler, const int* valid_len, int B, int N,
+                          int nt, int Td, cudaStream_t s) {
+  const int K = nt < N ? nt : N;
+  constexpr int kMaxTokens = 12288;  // the valid-row list of one sample in 48 KB of shared memory
+  if (K > kMaxTokens) {
+    set_error("text average upsampling: at most %d text tokens per sample (got %d)", kMaxTokens, K);
+    return -1;
+  }
+  constexpr int rows = 32;
+  text_avg_upsample_kernel<<<dim3(B, (N + rows - 1) / rows), 256, sizeof(int) * (K > 0 ? K : 1), s>>>(
+      tx, out, filler, valid_len, B, N, K, Td, rows);
+  count_launch();
+  return check_launch("text_avg_upsample_kernel");
+}
+
 int run_mask_rows(float* x, const uint8_t* filler, int BN, int rows, int C, cudaStream_t s) {
   mask_rows_kernel<<<rows, 128, 0, s>>>(x, filler, BN, rows, C);
   count_launch();

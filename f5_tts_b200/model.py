@@ -94,7 +94,7 @@ def _attach(root: nn.Module, dotted: str, tensor: torch.Tensor, buffer=False):
 
 
 def _backbone_spec(kind: str, *, dim, depth, heads, dim_head, ff_mult, mel_dim, text_num_embeds, text_dim,
-                   conv_layers):
+                   conv_layers, qk_norm=None, long_skip_connection=False):
     """(key, shape, init) for every tensor of the backbone; identical names to dit.py / unett.py modules."""
     D, T, Mel = dim, text_dim, mel_dim
     inner, ff = heads * dim_head, int(dim * ff_mult)
@@ -125,9 +125,13 @@ def _backbone_spec(kind: str, *, dim, depth, heads, dim_head, ff_mult, mel_dim, 
             lin(b + "attn_norm.linear", 6 * D, D, init="zero")  # AdaLN-Zero (dit.py:264-274)
             for nm in ("to_q", "to_k", "to_v"):
                 lin(b + "attn." + nm, inner, D)
+            if qk_norm is not None:  # RMSNorm(dim_head) gains (modules.py:406-407)
+                out += [(b + "attn.q_norm.weight", (dim_head,), "one"), (b + "attn.k_norm.weight", (dim_head,), "one")]
             lin(b + "attn.to_out.0", D, inner)
             lin(b + "ff.ff.0.0", ff, D)
             lin(b + "ff.ff.2", D, ff)
+        if long_skip_connection:  # dit.py:228
+            lin("long_skip_connection", D, 2 * D, bias=False)
         lin("norm_out.linear", 2 * D, D, init="zero")
         lin("proj_out", Mel, D, init="zero")
     else:
@@ -138,6 +142,8 @@ def _backbone_spec(kind: str, *, dim, depth, heads, dim_head, ff_mult, mel_dim, 
             out.append((b + "1.g", (D,), "one"))
             for nm in ("to_q", "to_k", "to_v"):
                 lin(b + "2." + nm, inner, D)
+            if qk_norm is not None:
+                out += [(b + "2.q_norm.weight", (dim_head,), "one"), (b + "2.k_norm.weight", (dim_head,), "one")]
             lin(b + "2.to_out.0", D, inner)
             out.append((b + "3.g", (D,), "one"))
             lin(b + "4.ff.0.0", ff, D)
@@ -173,14 +179,20 @@ class _Backbone(nn.Module):
                  text_num_embeds=256, text_dim=None, text_mask_padding=True, qk_norm=None, conv_layers=0,
                  pe_attn_head=None, attn_backend="torch", attn_mask_enabled=False, **unsupported):
         super().__init__()
-        if qk_norm is not None:
-            raise NotImplementedError("qk_norm is null in every shipped config (configs/*.yaml); not built")
-        for k in ("text_embedding_average_upsampling", "long_skip_connection", "checkpoint_activations"):
-            if unsupported.pop(k, False):
-                raise NotImplementedError(f"{k} is off in every shipped config; not built")
+        # DiT-only options (backbones/dit.py:180-186); UNetT's constructor does not take them (unett.py:109-128).
+        # checkpoint_activations only recomputes activations in training (dit.py:358-361): accepted and ignored.
+        avg_up = bool(unsupported.pop("text_embedding_average_upsampling", False))
+        long_skip = bool(unsupported.pop("long_skip_connection", False))
+        unsupported.pop("checkpoint_activations", None)
+        if self.KIND != "DiT" and (avg_up or long_skip):
+            raise TypeError("text_embedding_average_upsampling and long_skip_connection are DiT arguments")
+        if avg_up:  # the reference's TextEmbedding asserts it (dit.py:41-43)
+            assert text_mask_padding, "text_embedding_average_upsampling requires text_mask_padding to be True"
         skip = unsupported.pop("skip_connect_type", "concat")
         if skip != "concat":
             raise NotImplementedError("UNetT skip_connect_type other than 'concat' is not built")
+        if qk_norm not in (None, "rms_norm"):
+            raise ValueError(f"Unimplemented qk_norm: {qk_norm}")  # modules.py:408-409
         if unsupported:
             raise TypeError(f"unexpected arguments: {sorted(unsupported)}")
         if dim_head != 64:
@@ -193,9 +205,12 @@ class _Backbone(nn.Module):
         self.text_mask_padding, self.conv_layers = bool(text_mask_padding), conv_layers
         self.pe_attn_head, self.attn_mask_enabled = pe_attn_head, bool(attn_mask_enabled)
         self.attn_backend = attn_backend  # accepted for config compatibility; the H100 kernel is always used
+        # long_skip: the flag (`long_skip_connection` is the Linear's module name, as in dit.py:228)
+        self.qk_norm, self.long_skip, self.text_embedding_average_upsampling = qk_norm, long_skip, avg_up
         for key, shape, how in _backbone_spec(self.KIND, dim=dim, depth=depth, heads=heads, dim_head=dim_head,
                                               ff_mult=ff_mult, mel_dim=mel_dim, text_num_embeds=text_num_embeds,
-                                              text_dim=text_dim, conv_layers=conv_layers):
+                                              text_dim=text_dim, conv_layers=conv_layers, qk_norm=qk_norm,
+                                              long_skip_connection=long_skip):
             _attach(self, key, _init_tensor(shape, how))
         inv_freq = 1.0 / (10000 ** (torch.arange(0, dim_head, 2).float() / dim_head))
         _attach(self, "rotary_embed.inv_freq", inv_freq, buffer=True)

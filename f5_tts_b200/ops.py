@@ -10,8 +10,8 @@ from typing import Optional
 import torch
 
 from . import _lib
-from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_MISH, ACT_NONE, EPI_F16, EPI_F32, EPI_QKV_ROPE,  # noqa: F401
-                   EPI_RESID)
+from ._lib import (ACT_GELU_ERF, ACT_GELU_TANH, ACT_MISH, ACT_NONE, EPI_F16, EPI_F32, EPI_QKV_NORM_ROPE,  # noqa: F401
+                   EPI_QKV_ROPE, EPI_RESID)
 
 
 def _stream(t: torch.Tensor):
@@ -29,11 +29,12 @@ def _need_cuda(*ts):
 
 
 def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, epi=EPI_F16, act=ACT_NONE, bn=0, pair=0, resid=None, gate=None,
-           row_len=None, seq=0, rope=None, inner=0, pe_heads=0, out16b=False, static_w=False):
+           row_len=None, seq=0, rope=None, inner=0, pe_heads=0, out16b=False, static_w=False, qk_norm=None):
     """C = epilogue(a @ w.T).  a fp16 [M, K], w fp16 [N, K] (both contiguous).
     static_w: w is a model weight (not produced by the preceding kernel) -> its tiles may be prefetched early.
+    qk_norm: (q gain, k gain), fp32 [64] each, for EPI_QKV_NORM_ROPE.
 """
-    _need_cuda(a, w, bias, resid, gate)
+    _need_cuda(a, w, bias, resid, gate, *(qk_norm or ()))
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and a.is_contiguous() and w.is_contiguous()
     M, K = a.shape
     N = w.shape[0]
@@ -43,7 +44,7 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, epi=EPI_F16, act=ACT_
     g.bias = _ptr(bias)
     out = None
     out2 = None
-    if epi in (EPI_F16, EPI_QKV_ROPE):
+    if epi in (EPI_F16, EPI_QKV_ROPE, EPI_QKV_NORM_ROPE):
         out = torch.empty((M, N), dtype=torch.float16, device=a.device)
         g.out = out.data_ptr()
     elif epi == EPI_F32:
@@ -63,6 +64,8 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, epi=EPI_F16, act=ACT_
     if rope is not None:
         g.rope_cos, g.rope_sin = rope[0].data_ptr(), rope[1].data_ptr()
     g.inner, g.pe_heads = inner, pe_heads
+    if qk_norm is not None:
+        g.q_norm, g.k_norm = _ptr(qk_norm[0]), _ptr(qk_norm[1])
     g.weights_static = 1 if static_w else 0
     with torch.cuda.device(a.device):
         _lib.check(_lib.lib().f5_gemm(a.data_ptr(), w.data_ptr(), C.byref(g), _stream(a)), "f5_gemm")

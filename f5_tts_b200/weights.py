@@ -72,6 +72,8 @@ def packed_tensors(m) -> dict[str, torch.Tensor]:
             if (p + "0.weight") in sd:
                 T[q + "w_skip"] = _h(sd[p + "0.weight"])
             T[q + "g_attn"], T[q + "g_ff"] = _f(sd[p + "1.g"]), _f(sd[p + "3.g"])
+        if m.qk_norm is not None:
+            T[q + "q_norm_w"], T[q + "k_norm_w"] = _f(sd[a + "q_norm.weight"]), _f(sd[a + "k_norm.weight"])
     if dit:
         mw = [sd[f"transformer_blocks.{i}.attn_norm.linear.weight"] for i in range(depth)] + [sd["norm_out.linear.weight"]]
         mb = [sd[f"transformer_blocks.{i}.attn_norm.linear.bias"] for i in range(depth)] + [sd["norm_out.linear.bias"]]
@@ -79,6 +81,8 @@ def packed_tensors(m) -> dict[str, torch.Tensor]:
     else:
         T["g_out"] = _f(sd["norm_out.g"])
     T["out_w"], T["out_b"] = _h(sd["proj_out.weight"]), _f(sd["proj_out.bias"])
+    if m.long_skip:
+        T["long_skip_w"] = _h(sd["long_skip_connection.weight"])
     return T
 
 
@@ -101,7 +105,8 @@ def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
     layers = (_lib.LayerWeights * depth)()
     for i in range(depth):
         lw, q = layers[i], f"L{i}."
-        for name in ("w_qkv", "b_qkv", "w_out", "b_out", "w_ff1", "b_ff1", "w_ff2", "b_ff2", "w_skip", "g_attn", "g_ff"):
+        for name in ("w_qkv", "b_qkv", "w_out", "b_out", "w_ff1", "b_ff1", "w_ff2", "b_ff2", "w_skip", "g_attn", "g_ff",
+                     "q_norm_w", "k_norm_w"):
             setattr(lw, name, P(q + name))
     W.layers = C.cast(layers, C.POINTER(_lib.LayerWeights))
     if dit:
@@ -109,6 +114,7 @@ def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
     else:
         W.g_out = P("g_out")
     W.out_w, W.out_b = P("out_w"), P("out_b")
+    W.long_skip_w = P("long_skip_w")
 
     A = _lib.Arch()
     A.backbone = 0 if dit else 1
@@ -117,6 +123,9 @@ def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
     A.text_mask_padding = 1 if m.text_mask_padding else 0
     A.pe_attn_head = -1 if m.pe_attn_head is None else int(m.pe_attn_head)
     A.attn_mask_enabled = 1 if m.attn_mask_enabled else 0
+    A.qk_norm = 1 if m.qk_norm is not None else 0
+    A.long_skip = 1 if m.long_skip else 0
+    A.text_avg_upsample = 1 if m.text_embedding_average_upsampling else 0
     handle = C.c_void_p()
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().f5_engine_create(C.byref(A), C.byref(W), C.byref(handle)), "f5_engine_create")
@@ -139,6 +148,9 @@ def cache_key(ckpt_path: str, m) -> str:
     st = os.stat(ckpt_path)
     arch = (m.KIND, m.dim, m.depth, m.heads, m.dim_head, m.ff_inner, m.mel_dim, m.text_dim, m.text_num_embeds,
             m.conv_layers, m.text_mask_padding, m.pe_attn_head)
+    options = (m.qk_norm, m.long_skip, m.text_embedding_average_upsampling)
+    if any(options):  # appended only when an option is on: packed caches of other models keep their keys
+        arch += options
     raw = f"{os.path.abspath(ckpt_path)}|{st.st_size}|{st.st_mtime_ns}|{arch}|fmt{PACK_FORMAT}"
     return hashlib.sha256(raw.encode()).hexdigest()[:24]
 

@@ -36,7 +36,10 @@ unsigned long long f5_launch_count(void);
  * ------------------------------------------------------------------------------------------------------------ */
 
 enum { F5_ACT_NONE = 0, F5_ACT_GELU_TANH = 1, F5_ACT_GELU_ERF = 2, F5_ACT_MISH = 3 };
-enum { F5_EPI_F16 = 0, F5_EPI_F32 = 1, F5_EPI_RESID = 2, F5_EPI_QKV_ROPE = 3 };
+/* F5_EPI_QKV_NORM_ROPE: F5_EPI_QKV_ROPE with the reference's qk_norm="rms_norm" (model/modules.py:402-409, 492-496;
+ * RMSNorm modules.py:286-305) on every q and k head before RoPE: v * rsqrt(mean_head(v^2) + 1e-6) * gain[c % 64], in
+ * fp32, v = acc + bias.  Needs q_norm, k_norm, rope tables, seq and inner % 64 == 0.  Since f5_version() 105. */
+enum { F5_EPI_F16 = 0, F5_EPI_F32 = 1, F5_EPI_RESID = 2, F5_EPI_QKV_ROPE = 3, F5_EPI_QKV_NORM_ROPE = 4 };
 
 /* Fused linear: C = epilogue(A[M,K] . W[N,K]^T) — replaces nn.Linear (aten::addmm) call sites
  * model/modules.py:317,338,360-361,398-400 and, with conv_taps != 0, the grouped Conv1d(k=taps, groups=N/k,
@@ -72,6 +75,8 @@ typedef struct {
    * entirely (not loaded, multiplied or stored: their output rows keep whatever the buffer held).  Needs row_len and
    * seq.  The reference's counterpart is its masked mode (flash_attn_varlen / attn_mask, modules.py:513-540). */
   int skip_padded_tiles;
+  const float* q_norm;     /* QKV_NORM_ROPE: fp32 [64] RMSNorm gain of the q heads (attn.q_norm.weight) */
+  const float* k_norm;     /* QKV_NORM_ROPE: fp32 [64] RMSNorm gain of the k heads (attn.k_norm.weight) */
 } f5_gemm_args;
 int f5_gemm(const void* A, const void* W, const f5_gemm_args* args, f5_stream_t stream);
 /* Tile shape f5_gemm would run `args` with (after bn = 0 resolution): *bn tile width, *cta_pair always 0. */
@@ -130,6 +135,13 @@ typedef struct {
   int text_mask_padding; /* yaml arch.text_mask_padding */
   int pe_attn_head;      /* -1 = all heads */
   int attn_mask_enabled;
+  /* Since f5_version() 105; all 0 reproduce the earlier engine exactly. */
+  int qk_norm;           /* 1 = qk_norm="rms_norm": per-head RMSNorm of q and k before RoPE (modules.py:402-409,
+                            492-496); needs q_norm_w / k_norm_w in every layer */
+  int long_skip;         /* DiT long_skip_connection (backbones/dit.py:228, 354-365): x = long_skip_w .
+                            cat(x after the last block, x after the input embedding) before norm_out */
+  int text_avg_upsample; /* DiT text_embedding_average_upsampling (backbones/dit.py:41-84, 131-137): each sample's
+                            valid text tokens spread evenly over its audio length; needs text_mask_padding */
 } f5_arch;
 
 typedef struct {
@@ -139,6 +151,8 @@ typedef struct {
   const void* w_ff2; const float* b_ff2;   /* fp16 [D, F] */
   const void* w_skip;                      /* UNetT later half: fp16 [D, 2D], else NULL */
   const float* g_attn; const float* g_ff;  /* UNetT RMSNorm gains */
+  const float* q_norm_w; const float* k_norm_w; /* arch.qk_norm: fp32 [64] attn.q_norm / k_norm weight
+                                                   (modules.py:406-407), else NULL */
 } f5_layer_weights;
 
 typedef struct {
@@ -158,6 +172,8 @@ typedef struct {
   const f5_layer_weights* layers;             /* [depth] */
   const float* g_out;                         /* UNetT norm_out.g */
   const void* out_w; const float* out_b;      /* fp16 [mel, D] proj_out */
+  const void* long_skip_w;                    /* arch.long_skip: fp16 [D, 2D] long_skip_connection.weight
+                                                 (backbones/dit.py:228, no bias), else NULL */
 } f5_weights;
 
 typedef struct f5_engine f5_engine;

@@ -33,6 +33,10 @@ class ArchConfig:
     conv_layers: int = 4
     pe_attn_head: Optional[int] = 1
     attn_mask_enabled: bool = False
+    # architecture options off in every shipped config (backbones/dit.py:180-186; UNetT takes qk_norm only)
+    qk_norm: Optional[str] = None  # None | "rms_norm"
+    long_skip_connection: bool = False
+    text_embedding_average_upsampling: bool = False
 
     @property
     def tdim(self) -> int:
@@ -63,6 +67,15 @@ def f5tts_v1_small() -> ArchConfig:  # configs/F5TTS_v1_Small.yaml:26-36
 def e2tts_small() -> ArchConfig:  # configs/E2TTS_Small.yaml:25-31
     return ArchConfig(backbone="UNetT", dim=768, depth=20, heads=12, ff_mult=4, text_dim=None, conv_layers=0,
                       text_mask_padding=False, pe_attn_head=1)
+
+
+def f5tts_v1_base_qk_norm() -> ArchConfig:  # F5TTS_v1_Base with `qk_norm: rms_norm`
+    return ArchConfig(text_mask_padding=True, pe_attn_head=None, qk_norm="rms_norm")
+
+
+def f5tts_v1_base_all_options() -> ArchConfig:  # F5TTS_v1_Base with qk_norm, long skip and text average upsampling
+    return ArchConfig(text_mask_padding=True, pe_attn_head=None, qk_norm="rms_norm", long_skip_connection=True,
+                      text_embedding_average_upsampling=True)
 
 
 # ---------------------------------------------------------------------------
@@ -108,9 +121,14 @@ def state_dict_spec(cfg: ArchConfig) -> list[tuple[str, tuple[int, ...], str]]:
             lin(b + "attn_norm.linear", 6 * D, D, kind="adaln")
             for nm in ("to_q", "to_k", "to_v"):
                 lin(b + "attn." + nm, inner, D)
+            if cfg.qk_norm is not None:  # RMSNorm gains (modules.py:406-407); ones in the reference, drawn here
+                spec.append((b + "attn.q_norm.weight", (cfg.dim_head,), "ln_w"))
+                spec.append((b + "attn.k_norm.weight", (cfg.dim_head,), "ln_w"))
             lin(b + "attn.to_out.0", D, inner)
             lin(b + "ff.ff.0.0", ff, D)
             lin(b + "ff.ff.2", D, ff)
+        if cfg.long_skip_connection:  # dit.py:228
+            lin(p + "long_skip_connection", D, 2 * D, bias=False)
         lin(p + "norm_out.linear", 2 * D, D, kind="adaln")
         lin(p + "proj_out", M, D)
     elif cfg.backbone == "UNetT":
@@ -121,6 +139,9 @@ def state_dict_spec(cfg: ArchConfig) -> list[tuple[str, tuple[int, ...], str]]:
             spec.append((b + "1.g", (D,), "ln_w"))
             for nm in ("to_q", "to_k", "to_v"):
                 lin(b + "2." + nm, inner, D)
+            if cfg.qk_norm is not None:
+                spec.append((b + "2.q_norm.weight", (cfg.dim_head,), "ln_w"))
+                spec.append((b + "2.k_norm.weight", (cfg.dim_head,), "ln_w"))
             lin(b + "2.to_out.0", D, inner)
             spec.append((b + "3.g", (D,), "ln_w"))
             lin(b + "4.ff.0.0", ff, D)

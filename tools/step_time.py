@@ -5,7 +5,8 @@ STEP_ODE=<method>:<steps>[,<method>:<steps>...] times each ODE solver setting in
 STEP_ROUNDS=<n> repeats the whole list n times, alternating, so that settings are compared within one process
 (e.g. STEP_ODE=euler:32,midpoint:16 — both make 32 backbone evaluations).
 STEP_ARCH=<preset>[,<preset>...] (synthdata presets, default the workload's arch) times each architecture on the same
-inputs, alternating within every round (e.g. STEP_ARCH=f5tts_v1_base,f5tts_v1_small)."""
+inputs, alternating within every round (e.g. STEP_ARCH=f5tts_v1_base,f5tts_v1_small; the architecture options have
+presets too: STEP_ARCH=f5tts_v1_base,f5tts_v1_base_qk_norm,f5tts_v1_base_all_options)."""
 import os
 import subprocess
 import sys
@@ -14,6 +15,7 @@ import torch
 
 sys.path.insert(0, ".")
 import bench  # noqa: E402
+import synthdata as SD  # noqa: E402
 
 dev = "cuda:0"
 name = os.environ.get("STEP_WORKLOAD", "cfg2")
@@ -22,8 +24,31 @@ runs = [(m, int(s)) for m, s in (p.split(":") for p in os.environ.get("STEP_ODE"
 rounds = int(os.environ.get("STEP_ROUNDS", "1"))
 archs = os.environ.get("STEP_ARCH", w["arch"]).split(",")
 models = {}
+
+
+def build_with_options(arch_name):
+    """bench.build_gpu_model plus the architecture options of the preset (qk_norm, long skip, text upsampling)."""
+    import f5_tts_b200 as F5
+
+    cfg = getattr(SD, arch_name)()
+    model = F5.CFM(transformer=F5.DiT(dim=cfg.dim, depth=cfg.depth, heads=cfg.heads, ff_mult=cfg.ff_mult,
+                                      text_dim=cfg.text_dim, text_mask_padding=cfg.text_mask_padding,
+                                      conv_layers=cfg.conv_layers, pe_attn_head=cfg.pe_attn_head,
+                                      text_num_embeds=cfg.text_num_embeds, mel_dim=100, qk_norm=cfg.qk_norm,
+                                      long_skip_connection=cfg.long_skip_connection,
+                                      text_embedding_average_upsampling=cfg.text_embedding_average_upsampling),
+                   vocab_char_map=models["f5tts_v1_base"].vocab_char_map)
+    model.load_state_dict(SD.synthetic_state_dict(cfg, seed=1234), strict=True)
+    return model.to(dev)
+
+
+models["f5tts_v1_base"], voc, _ = bench.build_gpu_model("f5tts_v1_base", dev)  # also the vocoder and vocabulary
 for a in archs:
-    models[a], voc, _ = bench.build_gpu_model(a, dev)
+    c = getattr(SD, a)()
+    if c.qk_norm or c.long_skip_connection or c.text_embedding_average_upsampling:
+        models[a] = build_with_options(a)
+    elif a not in models:
+        models[a], voc, _ = bench.build_gpu_model(a, dev)
 wav, text, duration, lens = (t.to(dev) for t in bench.synth_inputs(w))
 try:
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
