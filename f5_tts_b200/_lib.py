@@ -27,7 +27,7 @@ class GemmArgs(C.Structure):
         ("gate", c_void_p), ("step_ptr", c_void_p), ("gate_step_stride", c_ll), ("row_len", c_void_p),
         ("seq", c_int), ("rope_cos", c_void_p), ("rope_sin", c_void_p), ("inner", c_int), ("pe_heads", c_int),
         ("weights_static", c_int),
-        ("skip_padded_tiles", c_int), ("q_norm", c_void_p), ("k_norm", c_void_p),
+        ("skip_padded_tiles", c_int), ("q_norm", c_void_p), ("k_norm", c_void_p), ("dim_head", c_int),
     ]
 
 
@@ -108,6 +108,7 @@ def lib():
         L.f5_gemm.argtypes = [c_void_p, c_void_p, C.POINTER(GemmArgs), c_void_p]
         L.f5_gemm_tile.argtypes = [C.POINTER(GemmArgs), C.POINTER(c_int), C.POINTER(c_int)]
         L.f5_attention.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_float, c_void_p]
+        L.f5_attention_dh.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p]
         L.f5_row_norm.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]
         L.f5_mel_spectrogram.argtypes = [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p]
         L.f5_vocos_workspace_bytes.argtypes = [c_int, c_int]
@@ -124,7 +125,7 @@ def lib():
         L.f5_sample.argtypes = [c_void_p, C.POINTER(SampleArgs), c_void_p, c_size_t, c_void_p]
         L.f5_sample_flops.argtypes = [c_void_p, c_int, c_int, c_int, c_float]
         L.f5_sample_flops.restype = C.c_double
-        for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_row_norm", "f5_mel_spectrogram", "f5_vocos_decode",
+        for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_row_norm", "f5_mel_spectrogram", "f5_vocos_decode",
                      "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample"):
             getattr(L, name).restype = c_int
         _lib = L
@@ -142,7 +143,8 @@ def launch_count() -> int:
 
 
 EXPORTED_SYMBOLS = [
-    "f5_version", "f5_last_error", "f5_launch_count", "f5_gemm", "f5_gemm_tile", "f5_attention", "f5_row_norm", "f5_mel_spectrogram",
+    "f5_version", "f5_last_error", "f5_launch_count", "f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh",
+    "f5_row_norm", "f5_mel_spectrogram",
     "f5_vocos_workspace_bytes", "f5_vocos_decode", "f5_vocos_decode_varlen", "f5_engine_create", "f5_engine_destroy",
     "f5_sample_workspace_bytes", "f5_sample", "f5_sample_flops",
 ]

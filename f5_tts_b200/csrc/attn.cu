@@ -1,16 +1,20 @@
-// Host side of the wgmma attention kernel + C entry point f5_attention.
+// Host side of the wgmma attention kernel + C entry points f5_attention (dim_head 64) and f5_attention_dh.
 #include "attn.cuh"
 #include "internal.h"
 
 namespace f5 {
 
-int attn_plan(AttnPlan* pl, const void* qkv, void* out, int batches, int seq, int heads, const int* kv_len,
-              float scale) {
+int attn_plan(AttnPlan* pl, const void* qkv, void* out, int batches, int seq, int heads, int dim_head,
+              const int* kv_len, float scale) {
   if (batches <= 0 || seq <= 0 || heads <= 0) {
     set_error("attention: empty problem");
     return -1;
   }
-  const int inner = heads * 64;
+  if (dim_head != 64 && dim_head != 128) {
+    set_error("attention: dim_head must be 64 or 128 (got %d)", dim_head);
+    return -1;
+  }
+  const int inner = heads * dim_head;
   const uint64_t dims[3] = {(uint64_t)3 * inner, (uint64_t)seq, (uint64_t)batches};
   const uint64_t strides[2] = {(uint64_t)3 * inner * 2, (uint64_t)seq * 3 * inner * 2};
   const uint32_t box[3] = {64, 128, 1};
@@ -24,31 +28,45 @@ int attn_plan(AttnPlan* pl, const void* qkv, void* out, int batches, int seq, in
   pl->p.scale_log2 = scale * 1.4426950408889634f;
   pl->p.out = reinterpret_cast<__half*>(out);
   pl->grid = dim3((seq + kAttnBQ - 1) / kAttnBQ, heads, batches);
+  pl->dh = dim_head;
+  return 0;
+}
+
+template <int DH>
+static int attn_configure_dh() {
+  if (int rc = check_cuda(cudaFuncSetAttribute(attn_fwd_wgmma_kernel<DH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)attn_smem_bytes(DH)),
+                          "cudaFuncSetAttribute(attn smem)"))
+    return rc;
+  cudaFuncSetAttribute(attn_fwd_wgmma_kernel<DH>, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
   return 0;
 }
 
 int attn_configure() {
-  if (int rc = check_cuda(cudaFuncSetAttribute(attn_fwd_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)kAttnSmem),
-                          "cudaFuncSetAttribute(attn smem)"))
-    return rc;
-  cudaFuncSetAttribute(attn_fwd_wgmma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-  return 0;
+  if (int rc = attn_configure_dh<64>()) return rc;
+  return attn_configure_dh<128>();
 }
 
 int attn_run(const AttnPlan& pl, cudaStream_t s) {
   if (int rc = configure_kernels()) return rc;
-  PdlLaunch L(pl.grid, dim3(kAttnThreads), kAttnSmem, s);
-  if (int rc = check_cuda(cudaLaunchKernelEx(&L.cfg, attn_fwd_wgmma_kernel, pl.tm, pl.p), "attention launch")) return rc;
+  PdlLaunch L(pl.grid, dim3(kAttnThreads), attn_smem_bytes(pl.dh), s);
+  const cudaError_t e = pl.dh == 128 ? cudaLaunchKernelEx(&L.cfg, attn_fwd_wgmma_kernel<128>, pl.tm, pl.p)
+                                     : cudaLaunchKernelEx(&L.cfg, attn_fwd_wgmma_kernel<64>, pl.tm, pl.p);
+  if (int rc = check_cuda(e, "attention launch")) return rc;
   count_launch();
   return check_launch("attn_fwd_wgmma_kernel launch");
 }
 
 }  // namespace f5
 
+extern "C" int f5_attention_dh(const void* qkv, void* out, int batches, int seq, int heads, int dim_head,
+                               const int* kv_len, float scale, f5_stream_t stream) {
+  f5::AttnPlan pl;
+  if (int rc = f5::attn_plan(&pl, qkv, out, batches, seq, heads, dim_head, kv_len, scale)) return rc;
+  return f5::attn_run(pl, reinterpret_cast<cudaStream_t>(stream));
+}
+
 extern "C" int f5_attention(const void* qkv, void* out, int batches, int seq, int heads, const int* kv_len, float scale,
                             f5_stream_t stream) {
-  f5::AttnPlan pl;
-  if (int rc = f5::attn_plan(&pl, qkv, out, batches, seq, heads, kv_len, scale)) return rc;
-  return f5::attn_run(pl, reinterpret_cast<cudaStream_t>(stream));
+  return f5_attention_dh(qkv, out, batches, seq, heads, 64, kv_len, scale, stream);
 }

@@ -1,17 +1,19 @@
-// Non-causal flash-attention forward on wgmma for dim_head = 64 (reference: model/modules.py:471-556,
-// F.scaled_dot_product_attention(q, k, v, attn_mask=None | key mask), scale 1/sqrt(64)).
+// Non-causal flash-attention forward on wgmma for dim_head DH = 64 or 128 (reference: model/modules.py:471-556,
+// F.scaled_dot_product_attention(q, k, v, attn_mask=None | key mask), scale 1/sqrt(DH)).
 //
 // One CTA = one (sample, head, 128-query block).  q/k/v are read in place from the fused QKV projection output
 // [Be*seq, 3*inner] (fp16) through ONE 3-D TMA tensor map (cols, seq rows, sample): no head-split transpose ever touches
-// HBM, and rows past the end of a sample are zero-filled by TMA instead of leaking the next sample.
+// HBM, and rows past the end of a sample are zero-filled by TMA instead of leaking the next sample.  A 128B-swizzled box
+// is at most 64 fp16 wide, so a 128-row tile of a head is DH / 64 boxes of 128 x 64 (16 KB each), one after the other.
 // Warp roles (288 threads): warps 0..7 = two consumer warpgroups, warpgroup g owns query rows [64 g, 64 g + 64);
 // warp 8 = TMA producer (Q once, then a kAttnStages-deep ring of K and V tiles of 128 keys).
-//   S = Q K^T   : wgmma m64n128k16 x 4, both operands K-major in shared memory, fp32 in registers
+//   S = Q K^T   : wgmma m64n128k16 x DH / 16, both operands K-major in shared memory, fp32 in registers
 //   softmax     : online max / sum in fp32 on the accumulator fragment (a row is spread over the four threads of a
 //                 quad: two shuffles per row max); exponentials with MUFU.EX2 in log2 units
 //   O += P V    : P is converted to packed fp16 in registers — the accumulator fragment of S has exactly the layout of
 //                 wgmma's register A operand, so P never touches shared memory — times V consumed MN-major straight
-//                 from its TMA layout (wgmma m64n64k16, transposed B)
+//                 from its TMA layout (wgmma m64nDHk16, transposed B; at DH = 128 the two 64-column boxes of V are the
+//                 two 64-wide MN blocks of the operand, kAttnTile bytes apart)
 // The two warpgroups run independently, so one's exponentials overlap the other's tensor-core work.
 #pragma once
 #include "common.cuh"
@@ -26,15 +28,19 @@ __device__ __forceinline__ float ex2_approx(float x) {  // one MUFU.EX2; -inf ->
   return y;
 }
 
+template <int DH>
 __global__ void __launch_bounds__(kAttnThreads, 1)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
+  static_assert(DH == 64 || DH == 128, "head width");
+  constexpr int BOXES = DH / 64;                   // 64-column TMA boxes per tile row
+  constexpr uint32_t TILE = kAttnTile * BOXES;     // one 128-row tile of q, k or v
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - smem_u32(smem_raw));
   uint8_t* sQ = smem;
-  uint8_t* sK = sQ + kAttnTile;                    // kAttnStages tiles
-  uint8_t* sV = sK + kAttnStages * kAttnTile;      // kAttnStages tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kAttnStages * kAttnTile);
+  uint8_t* sK = sQ + TILE;                         // kAttnStages tiles
+  uint8_t* sV = sK + kAttnStages * TILE;           // kAttnStages tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kAttnStages * TILE);
   uint64_t* q_full = bars;                         // [1]
   uint64_t* k_full = q_full + 1;                   // [stages]
   uint64_t* k_empty = k_full + kAttnStages;        // [stages]
@@ -44,7 +50,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
   const int warp = threadIdx.x >> 5;
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int q0 = qb * kAttnBQ;
-  const int col_q = h * 64, col_k = p.inner + h * 64, col_v = 2 * p.inner + h * 64;
+  const int col_q = h * DH, col_k = p.inner + h * DH, col_v = 2 * p.inner + h * DH;
 
   if (warp == 8 && elect_one()) {
     tma_prefetch_desc(&tmQKV);
@@ -66,17 +72,22 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
 
   if (warp == 8) {
     if (elect_one()) {
-      mbar_expect_tx(q_full, kAttnTile);
-      tma_load_3d(sQ, &tmQKV, q_full, col_q, q0, b);
+      mbar_expect_tx(q_full, TILE);
+#pragma unroll
+      for (int c = 0; c < BOXES; ++c) tma_load_3d(sQ + c * kAttnTile, &tmQKV, q_full, col_q + 64 * c, q0, b);
       for (int j = 0; j < n_kv; ++j) {
         const int s = j % kAttnStages;
         const uint32_t ph = (j / kAttnStages) & 1;
         mbar_wait(&k_empty[s], ph ^ 1);
-        mbar_expect_tx(&k_full[s], kAttnTile);
-        tma_load_3d(sK + s * kAttnTile, &tmQKV, &k_full[s], col_k, j * kAttnBKV, b);
+        mbar_expect_tx(&k_full[s], TILE);
+#pragma unroll
+        for (int c = 0; c < BOXES; ++c)
+          tma_load_3d(sK + s * TILE + c * kAttnTile, &tmQKV, &k_full[s], col_k + 64 * c, j * kAttnBKV, b);
         mbar_wait(&v_empty[s], ph ^ 1);
-        mbar_expect_tx(&v_full[s], kAttnTile);
-        tma_load_3d(sV + s * kAttnTile, &tmQKV, &v_full[s], col_v, j * kAttnBKV, b);
+        mbar_expect_tx(&v_full[s], TILE);
+#pragma unroll
+        for (int c = 0; c < BOXES; ++c)
+          tma_load_3d(sV + s * TILE + c * kAttnTile, &tmQKV, &v_full[s], col_v + 64 * c, j * kAttnBKV, b);
       }
     }
     return;
@@ -88,9 +99,9 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
   const int r = 64 * g + 16 * (warp & 3) + (lane >> 2);
   const int c2 = 2 * (lane & 3);
   const uint64_t qdesc = make_wgmma_desc_sw128(smem_u32(sQ + g * (64 * 128)));
-  float o[32];
+  float o[DH / 2];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.0f;
+  for (int i = 0; i < DH / 2; ++i) o[i] = 0.0f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.0f, 0.0f};  // l: this thread's partial row sums
   mbar_wait(q_full, 0);
   for (int j = 0; j < n_kv; ++j) {
@@ -99,10 +110,14 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     const int kv_rem = kv_len - j * kAttnBKV;  // valid keys in this tile (>= 1)
     float sc[64];
     mbar_wait(&k_full[s], ph);
-    const uint64_t kdesc = make_wgmma_desc_sw128(smem_u32(sK + s * kAttnTile));
+    const uint64_t kdesc = make_wgmma_desc_sw128(smem_u32(sK + s * TILE));
     wgmma_fence();
+    // k-step k: 16 columns of the head, in box k / 4 (kAttnTile bytes = kAttnTile >> 4 descriptor units further on)
 #pragma unroll
-    for (int k = 0; k < 4; ++k) wgmma_ss_n128(sc, qdesc + uint64_t(2 * k), kdesc + uint64_t(2 * k), k != 0);
+    for (int k = 0; k < DH / 16; ++k) {
+      const uint64_t off = uint64_t((k >> 2) * (kAttnTile >> 4) + 2 * (k & 3));
+      wgmma_ss_n128(sc, qdesc + off, kdesc + off, k != 0);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(sc);
@@ -136,7 +151,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
       l_run[hr] = l_run[hr] * alpha[hr] + sum;
     }
 #pragma unroll
-    for (int jj = 0; jj < 8; ++jj) {
+    for (int jj = 0; jj < DH / 8; ++jj) {
       o[4 * jj + 0] *= alpha[0];
       o[4 * jj + 1] *= alpha[0];
       o[4 * jj + 2] *= alpha[1];
@@ -154,8 +169,12 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     mbar_wait(&v_full[s], ph);
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk)  // B = 16 key rows of V (2 KB apart), MN-major
-      wgmma_rs_n64_bt(o, pa[kk], make_wgmma_desc_sw128(smem_u32(sV + s * kAttnTile + kk * 16 * 128)), 1);
+    for (int kk = 0; kk < 8; ++kk) {  // B = 16 key rows of V (2 KB apart), MN-major
+      if constexpr (DH == 64)
+        wgmma_rs_n64_bt(o, pa[kk], make_wgmma_desc_sw128(smem_u32(sV + s * TILE + kk * 16 * 128)), 1);
+      else
+        wgmma_rs_n128_bt(o, pa[kk], make_wgmma_desc_sw128_mn(smem_u32(sV + s * TILE + kk * 16 * 128), kAttnTile), 1);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(o);
@@ -171,9 +190,9 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     const float inv_l = 1.0f / l;
     const int qrow = q0 + r + 8 * hr;
     if (qrow < p.seq) {
-      __half* out = p.out + ((long long)b * p.seq + qrow) * p.inner + h * 64 + c2;
+      __half* out = p.out + ((long long)b * p.seq + qrow) * p.inner + h * DH + c2;
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj)
+      for (int jj = 0; jj < DH / 8; ++jj)
         *reinterpret_cast<uint32_t*>(out + 8 * jj) = pack_half2(o[4 * jj + 2 * hr] * inv_l, o[4 * jj + 2 * hr + 1] * inv_l);
     }
   }

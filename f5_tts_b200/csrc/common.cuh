@@ -108,6 +108,12 @@ __device__ __forceinline__ uint64_t make_wgmma_desc_sw128(uint32_t smem_addr) {
   d |= uint64_t(1) << 62;          // layout type 1 = SWIZZLE_128B
   return d;
 }
+// MN-major operand wider than one 64-element swizzle row: blocks of 64 MN elements lie `mn_block_bytes` apart (the
+// leading byte offset; canonical layout ((8 x 8, m), (8, k)) : ((1 x 8, LBO), (64, SBO)) in fp16 elements).
+__device__ __forceinline__ uint64_t make_wgmma_desc_sw128_mn(uint32_t smem_addr, uint32_t mn_block_bytes) {
+  uint64_t d = make_wgmma_desc_sw128(smem_addr) & ~(uint64_t(0x3FFF) << 16);
+  return d | (uint64_t((mn_block_bytes >> 4) & 0x3FFF) << 16);
+}
 
 // ----------------------------------------------------------------------------------------------
 // math

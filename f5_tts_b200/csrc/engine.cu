@@ -132,8 +132,8 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.io = bp.take<SampleIo>(1);
   L.stage = bp.take<OdeStage>(evals);
   L.t_dev = bp.take<float>(evals);
-  L.rope_cos = bp.take<float>((size_t)L.seq * 32);
-  L.rope_sin = bp.take<float>((size_t)L.seq * 32);
+  L.rope_cos = bp.take<float>((size_t)L.seq * (A.dim_head / 2));
+  L.rope_sin = bp.take<float>((size_t)L.seq * (A.dim_head / 2));
   L.row_len = bp.take<int>(L.Be);
   L.kv_len = bp.take<int>(L.Be);
   L.frame_len = bp.take<int>(L.Be);
@@ -184,8 +184,12 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
     set_error("engine_create: null argument");
     return -1;
   }
-  if (arch->dim_head != 64) {
-    set_error("engine_create: dim_head must be 64 (got %d)", arch->dim_head);
+  if (arch->dim_head != 64 && arch->dim_head != 128) {
+    set_error("engine_create: dim_head must be 64 or 128 (got %d)", arch->dim_head);
+    return -1;
+  }
+  if (arch->dim_head == 128 && arch->heads * 128 > 1024) {  // inner = heads * 128 is a multiple of 128
+    set_error("engine_create: at dim_head 128, heads * dim_head must be at most 1024 (heads=%d)", arch->heads);
     return -1;
   }
   if (arch->dim % 128 || arch->dim > 1024 || (arch->ff_inner % 64)) {
@@ -247,16 +251,19 @@ size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, floa
 double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
   const f5_arch& A = e->arch;
   const double D = A.dim, mel = A.mel_dim, Td = A.text_dim, F = A.ff_inner, Ld = A.depth;
+  // attention width heads * dim_head: QKV 6 n D I + out-projection 2 n I D, QK^T + PV 4 n^2 I.  At dim_head 64 the
+  // count keeps the form it always had (I = D, as in every shipped config), so figures reported before stay comparable.
+  const double I = A.dim_head == 64 ? D : double(e->inner);
   const double Be = cfg_strength < 1e-5f ? B : 2.0 * B;
   double per;  // one sample-forward
   if (A.backbone == 0) {
     const double n = N;
-    per = Ld * (8.0 * n * D * D + 4.0 * n * D * F + 4.0 * n * n * D) + 2.0 * n * (2 * mel + Td) * D +
+    per = Ld * (8.0 * n * D * I + 4.0 * n * D * F + 4.0 * n * n * I) + 2.0 * n * (2 * mel + Td) * D +
           2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n * D * mel;
     if (A.long_skip) per += 2.0 * n * D * (2.0 * D);  // long_skip_connection: Linear(2D -> D)
   } else {
     const double n1 = N + 1.0, n = N;
-    per = Ld * (8.0 * n1 * D * D + 4.0 * n1 * D * F + 4.0 * n1 * n1 * D) + (Ld / 2.0) * 4.0 * n1 * D * D +
+    per = Ld * (8.0 * n1 * D * I + 4.0 * n1 * D * F + 4.0 * n1 * n1 * I) + (Ld / 2.0) * 4.0 * n1 * D * D +
           2.0 * n * (2 * mel + Td) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n1 * D * mel;
   }
   double total = nfe * Be * per;
@@ -385,6 +392,7 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
       a.rope_sin = L.rope_sin;
       a.inner = inner;
       a.pe_heads = pe_heads;
+      a.dim_head = A.dim_head;
       varlen(a);
       RC(gemm_plan(&P.qkv[i], L.a, lw.w_qkv, &a));
     }
@@ -439,7 +447,7 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
     RC(gemm_plan(&P.out_proj, L.a, W.out_w, &a));
   }
   P.attn.resize(1);
-  RC(attn_plan(&P.attn[0], L.qkv, L.ao, L.Be, L.seq, A.heads, skip ? L.kv_len : nullptr,
+  RC(attn_plan(&P.attn[0], L.qkv, L.ao, L.Be, L.seq, A.heads, A.dim_head, skip ? L.kv_len : nullptr,
                1.0f / sqrtf((float)A.dim_head)));
   return 0;
 }
@@ -596,7 +604,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
       RC(check_cuda(cudaMemsetAsync(L.qkv, 0, sizeof(__half) * L.M1 * 3 * e->inner, s), "qkv clear"));
     }
   }
-  RC(run_rope_table(L.rope_cos, L.rope_sin, L.seq, 32, s));
+  RC(run_rope_table(L.rope_cos, L.rope_sin, L.seq, A.dim_head / 2, s));
   // time embedding for every evaluation time (modules.py:852-862)
   RC(run_time_features(L.t_dev, L.tfeat, S, 256, s));
   RC(run_small_linear(1, L.tfeat, reinterpret_cast<const __half*>(W.time_w0), W.time_b0, L.th1, S, 256, D, s));

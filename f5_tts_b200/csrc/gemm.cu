@@ -115,6 +115,12 @@ static const GemmKernel kGemmKernels[] = {
     F5_GEMM_KERNEL(128, EPI_QKV_NORM_ROPE, ACT_NONE, false),
     F5_GEMM_KERNEL(192, EPI_QKV_NORM_ROPE, ACT_NONE, false),
     F5_GEMM_KERNEL(256, EPI_QKV_NORM_ROPE, ACT_NONE, false),
+    // 128-column heads (f5_gemm_args.dim_head = 128).  QKV_NORM_ROPE is 128 wide only: a 192-wide tile would split a
+    // head, and the 256-wide one spills (24 bytes; DESIGN.md §4).
+    F5_GEMM_KERNEL(128, EPI_QKV_ROPE_DH128, ACT_NONE, false),
+    F5_GEMM_KERNEL(192, EPI_QKV_ROPE_DH128, ACT_NONE, false),
+    F5_GEMM_KERNEL(256, EPI_QKV_ROPE_DH128, ACT_NONE, false),
+    F5_GEMM_KERNEL(128, EPI_QKV_NORM_ROPE_DH128, ACT_NONE, false),
 };
 #undef F5_GEMM_KERNEL
 
@@ -231,13 +237,21 @@ static int pick_tile(long long rows, int batches, int n_out, int k, int epi, int
   return best;
 }
 
+// Epilogue of the kernel that runs `a`: the QKV epilogues over 128-column heads are instantiations of their own.
+static int kernel_epi(const f5_gemm_args* a) {
+  if (a->dim_head != 128) return a->epi;
+  return a->epi == F5_EPI_QKV_ROPE ? EPI_QKV_ROPE_DH128 : a->epi == F5_EPI_QKV_NORM_ROPE ? EPI_QKV_NORM_ROPE_DH128 : a->epi;
+}
+
 // Tile width f5_gemm runs `a` with: conv tiles are 64 wide, bn = 0 leaves the width to the planner.
 static int resolve_tile(const f5_gemm_args* a, int* bn) {
   if (a->cta_pair != 0) {
     set_error("gemm: cta_pair must be 0 (there are no cluster-pair tiles)");
     return -1;
   }
-  *bn = a->conv_taps > 0 ? 64 : a->bn != 0 ? a->bn : pick_tile(a->rows, a->batches, a->n_out, a->k, a->epi, a->act);
+  *bn = a->conv_taps > 0 ? 64
+        : a->bn != 0    ? a->bn
+                        : pick_tile(a->rows, a->batches, a->n_out, a->k, kernel_epi(a), a->act);
   return 0;
 }
 
@@ -254,6 +268,22 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     set_error("gemm: empty problem (rows=%d batches=%d n_out=%d)", a->rows, a->batches, a->n_out);
     return -1;
   }
+  const bool qkv_epi = a->epi == F5_EPI_QKV_ROPE || a->epi == F5_EPI_QKV_NORM_ROPE;
+  if (a->dim_head != 0 && a->dim_head != 64 && !(qkv_epi && a->dim_head == 128)) {
+    set_error("gemm: dim_head must be 0 (= 64), 64 or, with a QKV epilogue, 128 (got %d)", a->dim_head);
+    return -1;
+  }
+  if (a->dim_head == 128) {
+    if (a->inner <= 0 || a->inner % 128 || a->n_out % 128 || a->rope_cos == nullptr || a->rope_sin == nullptr ||
+        a->seq <= 0 || conv) {
+      set_error("gemm: QKV epilogues at dim_head 128 need inner %% 128 == 0, n_out %% 128 == 0, rope tables and seq");
+      return -1;
+    }
+    if (a->epi == F5_EPI_QKV_NORM_ROPE && bn != 128) {
+      set_error("gemm: QKV_NORM_ROPE at dim_head 128 runs with bn 128 only (got %d)", bn);
+      return -1;
+    }
+  }
   if (a->epi == F5_EPI_QKV_ROPE && (a->inner % 64 || a->rope_cos == nullptr || a->seq <= 0)) {
     set_error("gemm: QKV_ROPE needs inner %% 64 == 0, rope tables and seq");
     return -1;
@@ -265,7 +295,7 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
     return -1;
   }
   pl->bn = bn;
-  pl->epi = a->epi;
+  pl->epi = kernel_epi(a);
   pl->act = a->act;
   pl->conv = conv ? 1 : 0;
   GemmParams& p = pl->p;
@@ -354,7 +384,7 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 
 extern "C" {
 
-int f5_version(void) { return 105; }
+int f5_version(void) { return 106; }
 const char* f5_last_error(void) { return f5::g_err; }
 unsigned long long f5_launch_count(void) { return f5::g_launches.load(); }
 

@@ -6,7 +6,8 @@
 // together share the A row-panel in L2 and sweep W once).  Warp roles (288 threads):
 //   warps 0..7    two consumer warpgroups: warpgroup g computes rows [64 g, 64 g + 64) of the 128 x BN tile with
 //                 wgmma m64nBNk16 (both operands read from shared memory), then runs the fused bias / activation /
-//                 qk RMSNorm / RoPE / gate / mask epilogue straight from its accumulator registers
+//                 qk RMSNorm / RoPE (64- or 128-column heads) / gate / mask epilogue straight from its accumulator
+//                 registers
 //   warp 8        TMA producer (one elected lane): STAGES-deep ring of {A 128x64, W BNx64} fp16 tiles, SWIZZLE_128B.  It
 //                 runs ahead into the next tile's k-blocks while the consumers are in the epilogue.
 // Pipeline: smem full / empty mbarriers (TMA <-> wgmma); every consumer warp releases a slot once its MMAs retired.
@@ -69,8 +70,11 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
   // first column not stored: a CONV tile ends with its group.  Evaluated at each use, so the plain kernels compile
   // exactly as when they compared with p.n_out directly.
   auto n_end = [&]() { return CONV ? n0 + p.conv_g : p.n_out; };
-  constexpr bool NORM = EPI == EPI_QKV_NORM_ROPE;
-  constexpr bool QKV = EPI == EPI_QKV_ROPE || NORM;
+  constexpr bool NORM = EPI == EPI_QKV_NORM_ROPE || EPI == EPI_QKV_NORM_ROPE_DH128;
+  constexpr bool QKV = EPI == EPI_QKV_ROPE || EPI == EPI_QKV_ROPE_DH128 || NORM;
+  // head width of the QKV epilogues (columns of one q, k or v head)
+  constexpr int DH = (EPI == EPI_QKV_ROPE_DH128 || EPI == EPI_QKV_NORM_ROPE_DH128) ? 128 : 64;
+  constexpr int LOG_DH = DH == 128 ? 7 : 6;
   // chunk width: the widest whose loads fit beside the BN / 2 accumulators without spilling (ptxas caps a 288-thread
   // CTA at 168 registers per thread).  QKV_NORM_ROPE adds its bias before the chunks, which frees the bias registers.
   constexpr int CW = NORM ? (BN <= 128 ? 64 : BN == 192 ? 32 : 8)
@@ -102,16 +106,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
     const int nb = n0 + CW * cc;
     if (nb >= n_end()) break;
     // qk_norm, at the first chunk of a head: the bias goes into the head's accumulators here (the chunks below add none),
-    // then, for a q or k head, 1 / RMS over its 64 columns in fp32.  The head lies in this tile (BN, n0 and CW divide
-    // into 64-column heads); one row of it is spread over the 4 lanes of a quad, 16 values each, so one pass over the
-    // head's registers and two quad shuffles give the sum of squares.  Kept per head, not per tile: 16 live values for a
-    // 256-wide tile spill.
-    if (NORM && ((CW * cc) & 63) == 0) {
+    // then, for a q or k head, 1 / RMS over its DH columns in fp32.  The head lies in this tile (BN, n0 and CW divide
+    // into DH-column heads: at DH = 128 only the 128-wide tile is instantiated); one row of it is spread over the
+    // 4 lanes of a quad, DH / 4 values each, so one pass over the head's registers and two quad shuffles give the sum of
+    // squares.  Kept per head, not per tile: 16 live values for a 256-wide tile spill.
+    if (NORM && ((CW * cc) & (DH - 1)) == 0) {
       const int hb = (CW * cc) >> 3;  // first 8-column group of the head
       const bool qk = nb / p.inner < 2;  // the same for the whole warp
       float ss[2] = {0.0f, 0.0f};
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
+      for (int j = 0; j < DH / 8; ++j) {
         float2 b = make_float2(0.0f, 0.0f);
         if (p.bias != nullptr) b = __ldg(reinterpret_cast<const float2*>(p.bias + nb + 8 * j + c2));
 #pragma unroll
@@ -127,7 +131,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
       for (int h = 0; h < 2; ++h) {
         ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 1);
         ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], 2);
-        rinv[h] = rsqrtf(ss[h] * (1.0f / 64.0f) + 1e-6f);
+        rinv[h] = rsqrtf(ss[h] * (1.0f / float(DH)) + 1e-6f);
       }
     }
     if (NORM && !in[0] && !in[1]) continue;
@@ -152,15 +156,15 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
     bool rope = false, nrm = false;
     float rc[2][J], rs[2][J];
     float2 gn[J];
-    if (QKV) {  // inner % 64 == 0 and CW divides 64: a chunk lies in one head of one section
-      const int sec = nb / p.inner, head = (nb - sec * p.inner) >> 6;
+    if (QKV) {  // inner % DH == 0 and CW divides DH: a chunk lies in one head of one section
+      const int sec = nb / p.inner, head = (nb - sec * p.inner) >> LOG_DH;
       rope = sec < 2 && head < p.pe_heads;
       if (NORM) {
         nrm = sec < 2;
         if (nrm) {
           const float* gw = sec == 0 ? p.q_norm : p.k_norm;
 #pragma unroll
-          for (int j = 0; j < J; ++j) gn[j] = __ldg(reinterpret_cast<const float2*>(gw + (nb & 63) + 8 * j + c2));
+          for (int j = 0; j < J; ++j) gn[j] = __ldg(reinterpret_cast<const float2*>(gw + (nb & (DH - 1)) + 8 * j + c2));
         }
       }
       if (rope) {
@@ -168,9 +172,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
         for (int h = 0; h < 2; ++h)
 #pragma unroll
           for (int j = 0; j < J; ++j) {
-            const int pr = ((nb & 63) >> 1) + 4 * j + (c2 >> 1);
-            rc[h][j] = in[h] ? __ldg(p.rope_cos + (long long)pos[h] * 32 + pr) : 0.0f;
-            rs[h][j] = in[h] ? __ldg(p.rope_sin + (long long)pos[h] * 32 + pr) : 0.0f;
+            const int pr = ((nb & (DH - 1)) >> 1) + 4 * j + (c2 >> 1);
+            rc[h][j] = in[h] ? __ldg(p.rope_cos + (long long)pos[h] * (DH / 2) + pr) : 0.0f;
+            rs[h][j] = in[h] ? __ldg(p.rope_sin + (long long)pos[h] * (DH / 2) + pr) : 0.0f;
           }
       }
     }

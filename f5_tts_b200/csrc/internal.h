@@ -48,9 +48,10 @@ struct AttnPlan {
   CUtensorMap tm;
   AttnParams p;
   dim3 grid;
+  int dh;  // head width: 64 or 128
 };
-int attn_plan(AttnPlan* plan, const void* qkv, void* out, int batches, int seq, int heads, const int* kv_len,
-              float scale);
+int attn_plan(AttnPlan* plan, const void* qkv, void* out, int batches, int seq, int heads, int dim_head,
+              const int* kv_len, float scale);
 int attn_run(const AttnPlan& plan, cudaStream_t s);
 
 // fp16 tensor map of rank 2 to 4, 128B swizzle: dims[0] is contiguous, strides[i] is the byte stride of dims[i + 1],

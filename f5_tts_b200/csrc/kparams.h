@@ -14,6 +14,10 @@ enum : int {
   EPI_QKV_ROPE = 3,  // out16[m,n] = rope(acc + bias) for the first pe_heads heads of q,k; plain for the rest
   // as EPI_QKV_ROPE, with a per-head RMSNorm(64, eps 1e-6, gain q_norm / k_norm) on every q and k head before RoPE
   EPI_QKV_NORM_ROPE = 4,
+  // EPI_QKV_ROPE / EPI_QKV_NORM_ROPE over 128-column heads.  Kernel-internal: the C ABI selects them with
+  // f5_gemm_args.dim_head = 128.
+  EPI_QKV_ROPE_DH128 = 5,
+  EPI_QKV_NORM_ROPE_DH128 = 6,
 };
 
 struct GemmParams {
@@ -42,7 +46,7 @@ struct GemmParams {
 #ifdef F5_TRACE
   int diag_no_epi;  // instrumented build: skip the epilogue (nothing is stored) to time the main loop alone
 #endif
-  // EPI_QKV_NORM_ROPE: fp32 [64] RMSNorm gains of the q and k heads.  Last, so the other epilogues' kernels keep their
+  // EPI_QKV_NORM_ROPE: fp32 [dim_head] RMSNorm gains of the q and k heads.  Last, so the other epilogues' kernels keep their
   // parameter offsets.
   const float* q_norm;
   const float* k_norm;
@@ -56,7 +60,7 @@ struct AttnParams {
   int seq;            // tokens per sample
   int heads;
   int batches;        // packed batch Be
-  int inner;          // heads * 64
+  int inner;          // heads * dim_head
   const int* kv_len;  // [Be] valid keys per sample, or null (= seq)
   float scale_log2;   // softmax scale * log2(e)
   __half* out;        // [Be*seq, inner]
@@ -66,8 +70,11 @@ constexpr int kAttnThreads = 288;   // two softmax / MMA warpgroups (64 query ro
 constexpr int kAttnBQ = 128;        // query rows per CTA
 constexpr int kAttnBKV = 128;       // keys per tile
 constexpr int kAttnStages = 3;      // K and V rings
-constexpr uint32_t kAttnTile = 128 * 64 * 2;  // 16 KB
-// Q + K,V rings + alignment slack + barriers
-constexpr size_t kAttnSmem = size_t(kAttnTile) * (1 + 2 * kAttnStages) + 1024 + 256;
+constexpr uint32_t kAttnTile = 128 * 64 * 2;  // 16 KB: one 128-row x 64-column TMA box
+// Q + K,V rings + alignment slack + barriers, for head width dh (dh / 64 boxes per tile).  dh = 128 with three stages
+// is 7 x 32 KB + 1.25 KB = 225.25 KB of the 227 KB an H100 CTA may have (DESIGN.md §4).
+constexpr size_t attn_smem_bytes(int dh) { return size_t(kAttnTile) * (dh / 64) * (1 + 2 * kAttnStages) + 1024 + 256; }
+constexpr size_t kAttnSmem = attn_smem_bytes(64);
+static_assert(attn_smem_bytes(128) <= 227 * 1024, "dim_head 128 attention tiles exceed shared memory");
 
 }  // namespace f5

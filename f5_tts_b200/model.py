@@ -170,6 +170,9 @@ def _nfe(steps: int, method: str) -> int:
     return 2 * steps if method == "midpoint" else steps
 
 
+DIM_HEADS = (64, 128)  # attention head widths the kernels are built for
+
+
 class _Backbone(nn.Module):
     """Shared implementation of the `transformer(...)` operator seam (SURVEY.md §8b)."""
 
@@ -195,8 +198,11 @@ class _Backbone(nn.Module):
             raise ValueError(f"Unimplemented qk_norm: {qk_norm}")  # modules.py:408-409
         if unsupported:
             raise TypeError(f"unexpected arguments: {sorted(unsupported)}")
-        if dim_head != 64:
-            raise NotImplementedError("the attention kernel is built for dim_head == 64")
+        if dim_head not in DIM_HEADS:
+            raise NotImplementedError(f"dim_head={dim_head}: the attention kernel is built for dim_head in {DIM_HEADS}")
+        if dim_head == 128 and heads * dim_head > 1024:
+            raise NotImplementedError(f"heads * dim_head = {heads * dim_head}: at dim_head 128 the attention width is "
+                                      "at most 1024")
         if text_dim is None:
             text_dim = mel_dim
         self.dim, self.depth, self.heads, self.dim_head = dim, depth, heads, dim_head

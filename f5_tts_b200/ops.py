@@ -29,10 +29,12 @@ def _need_cuda(*ts):
 
 
 def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, epi=EPI_F16, act=ACT_NONE, bn=0, pair=0, resid=None, gate=None,
-           row_len=None, seq=0, rope=None, inner=0, pe_heads=0, out16b=False, static_w=False, qk_norm=None):
+           row_len=None, seq=0, rope=None, inner=0, pe_heads=0, out16b=False, static_w=False, qk_norm=None,
+           dim_head=64):
     """C = epilogue(a @ w.T).  a fp16 [M, K], w fp16 [N, K] (both contiguous).
     static_w: w is a model weight (not produced by the preceding kernel) -> its tiles may be prefetched early.
-    qk_norm: (q gain, k gain), fp32 [64] each, for EPI_QKV_NORM_ROPE.
+    qk_norm: (q gain, k gain), fp32 [dim_head] each, for EPI_QKV_NORM_ROPE.
+    dim_head: columns per head of the QKV epilogues, 64 or 128 (rope tables [seq, dim_head / 2]).
 """
     _need_cuda(a, w, bias, resid, gate, *(qk_norm or ()))
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and a.is_contiguous() and w.is_contiguous()
@@ -67,15 +69,17 @@ def linear(a: torch.Tensor, w: torch.Tensor, bias=None, *, epi=EPI_F16, act=ACT_
     if qk_norm is not None:
         g.q_norm, g.k_norm = _ptr(qk_norm[0]), _ptr(qk_norm[1])
     g.weights_static = 1 if static_w else 0
+    g.dim_head = dim_head
     with torch.cuda.device(a.device):
         _lib.check(_lib.lib().f5_gemm(a.data_ptr(), w.data_ptr(), C.byref(g), _stream(a)), "f5_gemm")
     return (out, out2) if out16b else out
 
 
-def gemm_tile(M: int, N: int, K: int, epi=EPI_F16, act=ACT_NONE, bn=0, pair=0):
+def gemm_tile(M: int, N: int, K: int, epi=EPI_F16, act=ACT_NONE, bn=0, pair=0, dim_head=64):
     """(tile width, cta_pair) the planner runs this GEMM shape with; cta_pair is always 0 (a non-zero `pair` raises)."""
     g = _lib.GemmArgs()
     g.rows, g.batches, g.n_out, g.k, g.bn, g.epi, g.act, g.cta_pair = M, 1, N, K, bn, epi, act, pair
+    g.dim_head = dim_head
     b, pr = C.c_int(0), C.c_int(0)
     _lib.check(_lib.lib().f5_gemm_tile(C.byref(g), C.byref(b), C.byref(pr)), "f5_gemm_tile")
     return b.value, pr.value
@@ -104,15 +108,23 @@ def grouped_conv31(x: torch.Tensor, w_packed: torch.Tensor, bias, *, resid=None,
     return out
 
 
-def attention(qkv: torch.Tensor, batches: int, seq: int, heads: int, kv_len=None, scale=None) -> torch.Tensor:
-    """qkv fp16 [batches*seq, 3*heads*64] -> fp16 [batches*seq, heads*64]"""
+def attention(qkv: torch.Tensor, batches: int, seq: int, heads: int, kv_len=None, scale=None,
+              dim_head=64) -> torch.Tensor:
+    """qkv fp16 [batches*seq, 3*heads*dim_head] -> fp16 [batches*seq, heads*dim_head]; dim_head 64 or 128, scale
+    1/sqrt(dim_head) by default"""
     _need_cuda(qkv, kv_len)
-    assert qkv.dtype == torch.float16 and qkv.is_contiguous() and qkv.shape == (batches * seq, 3 * heads * 64)
-    out = torch.empty((batches * seq, heads * 64), dtype=torch.float16, device=qkv.device)
-    scale = 0.125 if scale is None else scale
+    inner = heads * dim_head
+    assert qkv.dtype == torch.float16 and qkv.is_contiguous() and qkv.shape == (batches * seq, 3 * inner)
+    out = torch.empty((batches * seq, inner), dtype=torch.float16, device=qkv.device)
+    scale = dim_head ** -0.5 if scale is None else scale
+    L = _lib.lib()
     with torch.cuda.device(qkv.device):
-        _lib.check(_lib.lib().f5_attention(qkv.data_ptr(), out.data_ptr(), batches, seq, heads, _ptr(kv_len), scale,
-                                           _stream(qkv)), "f5_attention")
+        if dim_head == 64:
+            _lib.check(L.f5_attention(qkv.data_ptr(), out.data_ptr(), batches, seq, heads, _ptr(kv_len), scale,
+                                      _stream(qkv)), "f5_attention")
+        else:
+            _lib.check(L.f5_attention_dh(qkv.data_ptr(), out.data_ptr(), batches, seq, heads, dim_head, _ptr(kv_len),
+                                         scale, _stream(qkv)), "f5_attention_dh")
     return out
 
 

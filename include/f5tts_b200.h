@@ -66,7 +66,7 @@ typedef struct {
   long long gate_step_stride;
   const int* row_len;      /* per-sample valid rows (NULL = all) */
   int seq;                 /* rows per sample */
-  const float* rope_cos;   /* [seq, 32] */
+  const float* rope_cos;   /* [seq, dim_head / 2] */
   const float* rope_sin;
   int inner, pe_heads;
   int weights_static;      /* 1 = W was NOT written by the kernel preceding this call on the stream (model weights):
@@ -75,8 +75,12 @@ typedef struct {
    * entirely (not loaded, multiplied or stored: their output rows keep whatever the buffer held).  Needs row_len and
    * seq.  The reference's counterpart is its masked mode (flash_attn_varlen / attn_mask, modules.py:513-540). */
   int skip_padded_tiles;
-  const float* q_norm;     /* QKV_NORM_ROPE: fp32 [64] RMSNorm gain of the q heads (attn.q_norm.weight) */
-  const float* k_norm;     /* QKV_NORM_ROPE: fp32 [64] RMSNorm gain of the k heads (attn.k_norm.weight) */
+  const float* q_norm;     /* QKV_NORM_ROPE: fp32 [dim_head] RMSNorm gain of the q heads (attn.q_norm.weight) */
+  const float* k_norm;     /* QKV_NORM_ROPE: fp32 [dim_head] RMSNorm gain of the k heads (attn.k_norm.weight) */
+  /* QKV epilogues: columns per head, 0 (= 64), 64 or 128.  At 128, rope tables are [seq, 64], the RMSNorm gains
+   * [128], inner and n_out multiples of 128, and QKV_NORM_ROPE runs with bn 128 only (the planner picks it).  Any
+   * other epilogue takes 0 or 64.  Since f5_version() 106. */
+  int dim_head;
 } f5_gemm_args;
 int f5_gemm(const void* A, const void* W, const f5_gemm_args* args, f5_stream_t stream);
 /* Tile shape f5_gemm would run `args` with (after bn = 0 resolution): *bn tile width, *cta_pair always 0. */
@@ -84,9 +88,14 @@ int f5_gemm_tile(const f5_gemm_args* args, int* bn, int* cta_pair);
 
 /* Non-causal attention over the fused QKV buffer — replaces F.scaled_dot_product_attention at
  * model/modules.py:519 (attn_mask=None, or the key mask of modules.py:513-517 via kv_len).
- *   qkv fp16 [batches*seq, 3*heads*64]; out fp16 [batches*seq, heads*64]. dim_head must be 64. */
+ *   qkv fp16 [batches*seq, 3*heads*64]; out fp16 [batches*seq, heads*64]. dim_head is 64. */
 int f5_attention(const void* qkv, void* out, int batches, int seq, int heads, const int* kv_len, float scale,
                  f5_stream_t stream);
+/* f5_attention with the head width as an argument: dim_head 64 or 128 (anything else returns -1).
+ *   qkv fp16 [batches*seq, 3*heads*dim_head]; out fp16 [batches*seq, heads*dim_head]; the reference's scale is
+ *   1/sqrt(dim_head).  f5_attention(...) is f5_attention_dh(..., 64, ...).  Since f5_version() 106. */
+int f5_attention_dh(const void* qkv, void* out, int batches, int seq, int heads, int dim_head, const int* kv_len,
+                    float scale, f5_stream_t stream);
 
 /* Row normalisation + modulation -> fp16 (model/modules.py:312-326,333-347,753; x_transformers RMSNorm unett.py:154)
  *   mode 0: LN(eps) * (1 + a[c]) + b[c]   mode 1: LN(eps) * a[c] + b[c]   mode 2: x/||x|| * sqrt(D) * a[c] */
@@ -131,6 +140,8 @@ int f5_vocos_decode_varlen(const f5_vocos_weights* w, const float* mel, int B, i
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct {
   int backbone;          /* 0 = DiT, 1 = UNetT */
+  /* dim_head: 64, or since f5_version() 106 also 128 (rope over the full head, softmax scale 1/sqrt(dim_head));
+   * heads * dim_head must be a multiple of 128 and at most 1024 at dim_head 128 */
   int dim, depth, heads, dim_head, ff_inner, mel_dim, text_dim, text_num_embeds, conv_layers;
   int text_mask_padding; /* yaml arch.text_mask_padding */
   int pe_attn_head;      /* -1 = all heads */
@@ -151,7 +162,7 @@ typedef struct {
   const void* w_ff2; const float* b_ff2;   /* fp16 [D, F] */
   const void* w_skip;                      /* UNetT later half: fp16 [D, 2D], else NULL */
   const float* g_attn; const float* g_ff;  /* UNetT RMSNorm gains */
-  const float* q_norm_w; const float* k_norm_w; /* arch.qk_norm: fp32 [64] attn.q_norm / k_norm weight
+  const float* q_norm_w; const float* k_norm_w; /* arch.qk_norm: fp32 [dim_head] attn.q_norm / k_norm weight
                                                    (modules.py:406-407), else NULL */
 } f5_layer_weights;
 

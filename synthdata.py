@@ -78,6 +78,10 @@ def f5tts_v1_base_all_options() -> ArchConfig:  # F5TTS_v1_Base with qk_norm, lo
                       text_embedding_average_upsampling=True)
 
 
+def f5tts_v1_base_dh128() -> ArchConfig:  # F5TTS_v1_Base with 8 heads of 128 (`heads: 8, dim_head: 128`)
+    return ArchConfig(text_mask_padding=True, pe_attn_head=None, heads=8, dim_head=128)
+
+
 # ---------------------------------------------------------------------------
 # synthetic weights in the released checkpoint layout
 # ---------------------------------------------------------------------------

@@ -6,7 +6,8 @@ STEP_ROUNDS=<n> repeats the whole list n times, alternating, so that settings ar
 (e.g. STEP_ODE=euler:32,midpoint:16 — both make 32 backbone evaluations).
 STEP_ARCH=<preset>[,<preset>...] (synthdata presets, default the workload's arch) times each architecture on the same
 inputs, alternating within every round (e.g. STEP_ARCH=f5tts_v1_base,f5tts_v1_small; the architecture options have
-presets too: STEP_ARCH=f5tts_v1_base,f5tts_v1_base_qk_norm,f5tts_v1_base_all_options)."""
+presets too: STEP_ARCH=f5tts_v1_base,f5tts_v1_base_qk_norm,f5tts_v1_base_all_options, and so do 128-wide heads:
+STEP_ARCH=f5tts_v1_base,f5tts_v1_base_dh128)."""
 import os
 import subprocess
 import sys
@@ -27,11 +28,13 @@ models = {}
 
 
 def build_with_options(arch_name):
-    """bench.build_gpu_model plus the architecture options of the preset (qk_norm, long skip, text upsampling)."""
+    """bench.build_gpu_model plus the architecture options of the preset (qk_norm, long skip, text upsampling) and its
+    head width."""
     import f5_tts_b200 as F5
 
     cfg = getattr(SD, arch_name)()
-    model = F5.CFM(transformer=F5.DiT(dim=cfg.dim, depth=cfg.depth, heads=cfg.heads, ff_mult=cfg.ff_mult,
+    model = F5.CFM(transformer=F5.DiT(dim=cfg.dim, depth=cfg.depth, heads=cfg.heads, dim_head=cfg.dim_head,
+                                      ff_mult=cfg.ff_mult,
                                       text_dim=cfg.text_dim, text_mask_padding=cfg.text_mask_padding,
                                       conv_layers=cfg.conv_layers, pe_attn_head=cfg.pe_attn_head,
                                       text_num_embeds=cfg.text_num_embeds, mel_dim=100, qk_norm=cfg.qk_norm,
@@ -45,7 +48,7 @@ def build_with_options(arch_name):
 models["f5tts_v1_base"], voc, _ = bench.build_gpu_model("f5tts_v1_base", dev)  # also the vocoder and vocabulary
 for a in archs:
     c = getattr(SD, a)()
-    if c.qk_norm or c.long_skip_connection or c.text_embedding_average_upsampling:
+    if c.qk_norm or c.long_skip_connection or c.text_embedding_average_upsampling or c.dim_head != 64:
         models[a] = build_with_options(a)
     elif a not in models:
         models[a], voc, _ = bench.build_gpu_model(a, dev)
