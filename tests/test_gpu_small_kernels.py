@@ -26,6 +26,7 @@ if not torch.cuda.is_available():
 
 from f5_tts_b200 import _lib, ops  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
+from oracle.kernel_bounds import assert_half, assert_within, ulp16  # noqa: E402,F401
 
 DEV = "cuda:0"
 U = 2.0 ** -24
@@ -88,30 +89,6 @@ def launch(name, *args):
 def rnd(shape, seed, scale=1.0, dtype=torch.float32):
     g = torch.Generator().manual_seed(seed)
     return (torch.randn(shape, generator=g, dtype=F64) * scale).to(dtype).to(DEV)
-
-
-def ulp16(x):
-    """fp16 ulp at |x| (subnormal spacing 2^-24 below 2^-14)."""
-    e = torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -14)))
-    return torch.pow(2.0, e - 10)
-
-
-def assert_within(got, ref, bound, what):
-    got, ref = got.to(F64), ref.to(F64)
-    err = (got - ref).abs()
-    bad = ~(err <= bound)  # also catches NaN
-    if bool(bad.any()):
-        i = int(torch.nonzero(bad.flatten())[0])
-        raise AssertionError(f"{what}: {int(bad.sum())} of {bad.numel()} elements outside the bound; first at flat index "
-                             f"{i}: got {float(got.flatten()[i])!r} ref {float(ref.flatten()[i])!r} "
-                             f"bound {float(bound.flatten()[i]):.3e}")
-    return float((err / bound.clamp_min(1e-300)).max()) if err.numel() else 0.0
-
-
-def assert_half(got, ref, e32, what):
-    """fp16 result: the fp32 bound plus half an fp16 ulp (taken at |ref| + e32, which covers a rounding across a binade)."""
-    assert got.dtype == torch.float16
-    return assert_within(got, ref, e32 + 0.5 * ulp16(ref.abs() + e32), what)
 
 
 def assert_equal(got, ref, what):
