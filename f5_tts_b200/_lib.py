@@ -52,6 +52,11 @@ class LayerWeights(C.Structure):
                                         "w_skip", "g_attn", "g_ff", "q_norm_w", "k_norm_w")]
 
 
+class CtxLayerWeights(C.Structure):  # f5_ctx_layer_weights: MMDiT text stream of one block
+    _fields_ = [(n, c_void_p) for n in ("w_qkv_c", "b_qkv_c", "w_out_c", "b_out_c", "w_ff1_c", "b_ff1_c", "w_ff2_c",
+                                        "b_ff2_c", "q_norm_c", "k_norm_c")]
+
+
 class TextBlock(C.Structure):
     _fields_ = [(n, c_void_p) for n in ("dw_w", "dw_b", "ln_w", "ln_b", "pw1_w", "pw1_b", "grn_gamma", "grn_beta",
                                         "pw2_w", "pw2_b")]
@@ -65,7 +70,7 @@ class Weights(C.Structure):
         ("conv_w", c_void_p * 2), ("conv_b", c_void_p * 2),
         ("mod_w", c_void_p), ("mod_b", c_void_p),
         ("layers", C.POINTER(LayerWeights)), ("g_out", c_void_p), ("out_w", c_void_p), ("out_b", c_void_p),
-        ("long_skip_w", c_void_p),
+        ("long_skip_w", c_void_p), ("ctx_layers", C.POINTER(CtxLayerWeights)),
     ]
 
 
@@ -78,7 +83,8 @@ class SampleArgs(C.Structure):
     ]
 
 
-ODE_METHODS = {"euler": 0, "midpoint": 1}  # SampleArgs.method; backbone evaluations per grid interval: 1 and 2
+ODE_METHODS = {"euler": 0, "midpoint": 1}
+BACKBONES = {"DiT": 0, "UNetT": 1, "MMDiT": 2}  # Arch.backbone  # SampleArgs.method; backbone evaluations per grid interval: 1 and 2
 
 
 _lock = threading.Lock()
@@ -109,6 +115,8 @@ def lib():
         L.f5_gemm_tile.argtypes = [C.POINTER(GemmArgs), C.POINTER(c_int), C.POINTER(c_int)]
         L.f5_attention.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_float, c_void_p]
         L.f5_attention_dh.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p]
+        L.f5_attention_joint.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                         c_void_p, c_void_p, c_int, c_float, c_void_p]
         L.f5_row_norm.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]
         L.f5_mel_spectrogram.argtypes = [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p]
         L.f5_vocos_workspace_bytes.argtypes = [c_int, c_int]
@@ -125,7 +133,12 @@ def lib():
         L.f5_sample.argtypes = [c_void_p, C.POINTER(SampleArgs), c_void_p, c_size_t, c_void_p]
         L.f5_sample_flops.argtypes = [c_void_p, c_int, c_int, c_int, c_float]
         L.f5_sample_flops.restype = C.c_double
-        for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_row_norm", "f5_mel_spectrogram", "f5_vocos_decode",
+        L.f5_sample_workspace_bytes_nt.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float]
+        L.f5_sample_workspace_bytes_nt.restype = c_size_t
+        L.f5_sample_flops_nt.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float]
+        L.f5_sample_flops_nt.restype = C.c_double
+        for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_attention_joint", "f5_row_norm", "f5_mel_spectrogram",
+                     "f5_vocos_decode",
                      "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample"):
             getattr(L, name).restype = c_int
         _lib = L
@@ -146,7 +159,8 @@ EXPORTED_SYMBOLS = [
     "f5_version", "f5_last_error", "f5_launch_count", "f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh",
     "f5_row_norm", "f5_mel_spectrogram",
     "f5_vocos_workspace_bytes", "f5_vocos_decode", "f5_vocos_decode_varlen", "f5_engine_create", "f5_engine_destroy",
-    "f5_sample_workspace_bytes", "f5_sample", "f5_sample_flops",
+    "f5_sample_workspace_bytes", "f5_sample", "f5_sample_flops", "f5_attention_joint", "f5_sample_workspace_bytes_nt",
+    "f5_sample_flops_nt",
 ]
 
 # Test-only library: the same objects plus one extern "C" wrapper per kernel launcher (csrc/kernel_hooks.cu), used by

@@ -28,9 +28,14 @@ __device__ __forceinline__ float ex2_approx(float x) {  // one MUFU.EX2; -inf ->
   return y;
 }
 
-template <int DH>
-__global__ void __launch_bounds__(kAttnThreads, 1)
-attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
+// JOINT (MMDiT joint attention, reference model/modules.py:563-705): queries and keys are [audio | text], the audio
+// segment read through tmQKV ([Be, seq, 3 inner]) and the text segment through tmC ([Be, jp.seq_c, 3 inner]).  Query
+// blocks [0, jp.q_blocks_a) are audio, the rest text; each writes its own segment's output.  The producer streams the
+// audio key tiles, then the text key tiles, through the same ring; the tail of each segment is masked on its own, so
+// every tile still holds at least one valid key.  A text segment with no valid keys contributes no tile.
+template <int DH, bool JOINT>
+__device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CUtensorMap* tmC, const AttnParams& p,
+                                              const AttnJointParams& jp) {
   static_assert(DH == 64 || DH == 128, "head width");
   constexpr int BOXES = DH / 64;                   // 64-column TMA boxes per tile row
   constexpr uint32_t TILE = kAttnTile * BOXES;     // one 128-row tile of q, k or v
@@ -49,11 +54,18 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
 
   const int warp = threadIdx.x >> 5;
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int q0 = qb * kAttnBQ;
+  bool text_q = false;  // JOINT: this CTA's queries are text rows
+  int q0 = qb * kAttnBQ;
+  if constexpr (JOINT) {
+    text_q = qb >= jp.q_blocks_a;
+    if (text_q) q0 = (qb - jp.q_blocks_a) * kAttnBQ;
+  }
+  const CUtensorMap* tmQ = text_q ? tmC : tmQKV;
   const int col_q = h * DH, col_k = p.inner + h * DH, col_v = 2 * p.inner + h * DH;
 
   if (warp == 8 && elect_one()) {
-    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(tmQKV);
+    if constexpr (JOINT) tma_prefetch_desc(tmC);
     mbar_init(q_full, 1);
     for (int s = 0; s < kAttnStages; ++s) {
       mbar_init(&k_full[s], 1);
@@ -68,26 +80,52 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
   pdl_launch_dependents();
   // a sample always has at least one key: kv_len < 1 (caller error on the public entry point) is treated as 1
   const int kv_len = p.kv_len ? max(1, min(p.kv_len[b], p.seq)) : p.seq;
-  const int n_kv = (kv_len + kAttnBKV - 1) / kAttnBKV;
+  int n_kv = (kv_len + kAttnBKV - 1) / kAttnBKV;
+  const int n_kv_a = n_kv;  // JOINT: tiles [n_kv_a, n_kv) are text keys
+  int kv_len_c = 0;
+  if constexpr (JOINT) {
+    kv_len_c = jp.c_len ? max(0, min(jp.c_len[b], jp.seq_c)) : jp.seq_c;
+    n_kv += (kv_len_c + kAttnBKV - 1) / kAttnBKV;
+  }
 
   if (warp == 8) {
     if (elect_one()) {
       mbar_expect_tx(q_full, TILE);
 #pragma unroll
-      for (int c = 0; c < BOXES; ++c) tma_load_3d(sQ + c * kAttnTile, &tmQKV, q_full, col_q + 64 * c, q0, b);
-      for (int j = 0; j < n_kv; ++j) {
-        const int s = j % kAttnStages;
-        const uint32_t ph = (j / kAttnStages) & 1;
-        mbar_wait(&k_empty[s], ph ^ 1);
-        mbar_expect_tx(&k_full[s], TILE);
+      for (int c = 0; c < BOXES; ++c) tma_load_3d(sQ + c * kAttnTile, tmQ, q_full, col_q + 64 * c, q0, b);
+      if constexpr (JOINT) {
+        for (int j = 0; j < n_kv; ++j) {
+          const int s = j % kAttnStages;
+          const uint32_t ph = (j / kAttnStages) & 1;
+          const bool text_kv = j >= n_kv_a;
+          const CUtensorMap* tmKV = text_kv ? tmC : tmQKV;
+          const int k0 = (text_kv ? j - n_kv_a : j) * kAttnBKV;
+          mbar_wait(&k_empty[s], ph ^ 1);
+          mbar_expect_tx(&k_full[s], TILE);
 #pragma unroll
-        for (int c = 0; c < BOXES; ++c)
-          tma_load_3d(sK + s * TILE + c * kAttnTile, &tmQKV, &k_full[s], col_k + 64 * c, j * kAttnBKV, b);
-        mbar_wait(&v_empty[s], ph ^ 1);
-        mbar_expect_tx(&v_full[s], TILE);
+          for (int c = 0; c < BOXES; ++c)
+            tma_load_3d(sK + s * TILE + c * kAttnTile, tmKV, &k_full[s], col_k + 64 * c, k0, b);
+          mbar_wait(&v_empty[s], ph ^ 1);
+          mbar_expect_tx(&v_full[s], TILE);
 #pragma unroll
-        for (int c = 0; c < BOXES; ++c)
-          tma_load_3d(sV + s * TILE + c * kAttnTile, &tmQKV, &v_full[s], col_v + 64 * c, j * kAttnBKV, b);
+          for (int c = 0; c < BOXES; ++c)
+            tma_load_3d(sV + s * TILE + c * kAttnTile, tmKV, &v_full[s], col_v + 64 * c, k0, b);
+        }
+      } else {
+        for (int j = 0; j < n_kv; ++j) {
+          const int s = j % kAttnStages;
+          const uint32_t ph = (j / kAttnStages) & 1;
+          mbar_wait(&k_empty[s], ph ^ 1);
+          mbar_expect_tx(&k_full[s], TILE);
+#pragma unroll
+          for (int c = 0; c < BOXES; ++c)
+            tma_load_3d(sK + s * TILE + c * kAttnTile, tmQKV, &k_full[s], col_k + 64 * c, j * kAttnBKV, b);
+          mbar_wait(&v_empty[s], ph ^ 1);
+          mbar_expect_tx(&v_full[s], TILE);
+#pragma unroll
+          for (int c = 0; c < BOXES; ++c)
+            tma_load_3d(sV + s * TILE + c * kAttnTile, tmQKV, &v_full[s], col_v + 64 * c, j * kAttnBKV, b);
+        }
       }
     }
     return;
@@ -107,7 +145,10 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
   for (int j = 0; j < n_kv; ++j) {
     const int s = j % kAttnStages;
     const uint32_t ph = (j / kAttnStages) & 1;
-    const int kv_rem = kv_len - j * kAttnBKV;  // valid keys in this tile (>= 1)
+    int kv_rem = kv_len - j * kAttnBKV;  // valid keys in this tile (>= 1)
+    if constexpr (JOINT) {
+      if (j >= n_kv_a) kv_rem = kv_len_c - (j - n_kv_a) * kAttnBKV;
+    }
     float sc[64];
     mbar_wait(&k_full[s], ph);
     const uint64_t kdesc = make_wgmma_desc_sw128(smem_u32(sK + s * TILE));
@@ -189,13 +230,27 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParam
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv_l = 1.0f / l;
     const int qrow = q0 + r + 8 * hr;
-    if (qrow < p.seq) {
-      __half* out = p.out + ((long long)b * p.seq + qrow) * p.inner + h * DH + c2;
+    const int seq_o = text_q ? jp.seq_c : p.seq;
+    if (qrow < seq_o) {
+      __half* out = (text_q ? jp.out_c : p.out) + ((long long)b * seq_o + qrow) * p.inner + h * DH + c2;
 #pragma unroll
       for (int jj = 0; jj < DH / 8; ++jj)
         *reinterpret_cast<uint32_t*>(out + 8 * jj) = pack_half2(o[4 * jj + 2 * hr] * inv_l, o[4 * jj + 2 * hr + 1] * inv_l);
     }
   }
+}
+
+template <int DH>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
+  attn_fwd_body<DH, false>(&tmQKV, &tmQKV, p, AttnJointParams{});
+}
+
+template <int DH>
+__global__ void __launch_bounds__(kAttnThreads, 1)
+attn_joint_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmC,
+                        const AttnParams p, const AttnJointParams jp) {
+  attn_fwd_body<DH, true>(&tmQKV, &tmC, p, jp);
 }
 
 }  // namespace f5

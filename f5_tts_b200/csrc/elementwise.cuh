@@ -170,6 +170,39 @@ __global__ void text_gather_kernel(const TextGatherParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// MMDiT text embedding (backbones/mmdit.py:31-63), both CFG variants: row = (variant, b, n) over Be*nt, variant 1 =
+// drop_text (all-zero ids).  c = table[id + 1] + sinus(min(n, 1023)) (precompute_freqs_cis(D, 1024),
+// get_pos_embed_indices clamps at 1023), zeroed where the id is -1 when mask_padding (the mask of the real text, for
+// both variants).  Text is not padded to N.  Also c_len[variant * B + b] = number of ids of sample b that are not -1.
+// ids [B, nt]; table fp32 [V+1, D]; out fp32 [Be*nt, D]; c_len [Be].
+// ---------------------------------------------------------------------------------------------------------
+__global__ void mmdit_text_embed_kernel(const long long* ids, int B, int nt, int D, const float* table, int num_embeds,
+                                        int mask_padding, float* out, int* c_len) {
+  const int row = blockIdx.x;
+  const int variant = row / (B * nt);
+  const int r = row % (B * nt);
+  const int b = r / nt, n = r % nt;
+  const long long raw = ids[r];
+  long long id = variant == 0 ? raw + 1 : 0;
+  id = id < 0 ? 0 : (id >= num_embeds ? num_embeds - 1 : id);  // never read outside the table
+  const bool zero = mask_padding && raw == -1;
+  const int pos = n < 1023 ? n : 1023;
+  const int half = D / 2;
+  for (int c = threadIdx.x; c < D; c += blockDim.x) {
+    const int i = c < half ? c : c - half;
+    const float freq = 1.0f / powf(10000.0f, float(2 * i) / float(D));
+    const float ang = float(pos) * freq;
+    const float v = table[id * D + c] + ((c < half) ? cosf(ang) : sinf(ang));
+    out[(long long)row * D + c] = zero ? 0.f : v;
+  }
+  if (n == 0 && threadIdx.x == 0) {
+    int cnt = 0;
+    for (int t = 0; t < nt; ++t) cnt += ids[(long long)b * nt + t] != -1;
+    c_len[variant * B + b] = cnt;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // text_embedding_average_upsampling (backbones/dit.py:55-84, 131-137): sample b's T valid text rows (filler == 0, the
 // cond variant's mask for both variants) are spread over its A audio rows, token j repeated A / T times plus once
 // more for the last A % T tokens; rows at or past A, and every row when T == 0, are 0.  A = valid_len[b], or N.

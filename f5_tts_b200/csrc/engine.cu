@@ -1,5 +1,6 @@
-// Engine: the CFM.sample NFE loop (model/cfm.py:160-223) over a DiT (backbones/dit.py:319-370) or UNetT
-// (backbones/unett.py:244-307) backbone, expressed as a fixed kernel schedule over a caller-owned workspace.
+// Engine: the CFM.sample NFE loop (model/cfm.py:160-223) over a DiT (backbones/dit.py:319-370), UNetT
+// (backbones/unett.py:244-307) or MMDiT (backbones/mmdit.py:198-246) backbone, expressed as a fixed kernel schedule over a
+// caller-owned workspace.
 //
 // The ODE solver is torchdiffeq's fixed-grid Euler (one backbone evaluation per grid interval, at t_k) or midpoint
 // (two: at t_k, then at t_k + dt_k/2 from the half-step state).  `evals` below counts backbone evaluations (NFE):
@@ -13,9 +14,13 @@
 // Per evaluation: input projection -> grouped conv position embedding x2 (tensor-core implicit GEMM) -> depth x
 // {norm+modulate, fused QKV+RoPE GEMM, flash attention, out-proj (+gate, +mask, +residual), norm+modulate,
 //  FF1+GELU, FF2 (+gate, +residual)} -> final norm -> proj_out -> fused CFG + ODE stage update.
+// MMDiT keeps a second residual stream for the text (c, [Be*nt, D]): per block both streams are normalised and projected
+// to QKV, one joint attention runs over [audio | text], and each stream has its own gated out-projection and FF pair (the
+// last block computes only the text QKV its audio queries attend to).
 // Every kernel reads the evaluation index from a device counter, so one captured CUDA graph serves all evaluations
 // of either method: the method reaches the graph only through the tables the prologue writes.
 #include <cmath>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -73,6 +78,12 @@ struct Layout {
   float* v;
   float* x_embed;  // DiT long_skip_connection: x after the input embedding [M1, D] (cat(...) goes to `cat`), else null
   float* txu;      // text_embedding_average_upsampling: upsampled text [2B, N, Td], else null
+  // MMDiT text stream (null for DiT / UNetT): nt tokens per sample
+  int nt;
+  float *c, *c0;               // [Be*nt, D] residual; the text embedding it restarts from at every evaluation
+  __half *ac, *qkv_c, *ao_c, *g_c;  // normalised copy, QKV, attention output, FF hidden
+  float *c_rope_cos, *c_rope_sin;   // [nt, dim_head / 2]
+  int* c_len;                  // [Be] valid text tokens per sample
   size_t bytes;
 };
 
@@ -98,8 +109,11 @@ struct GraphHolder {
 struct GraphKey {
   const void* ws;
   int B, N, evals, packed, masked;  // masked: 0 = no lengths, 1 = lengths (reference batched semantics), 2 = exact_varlen
+  int nt;  // MMDiT: the text length sets the text-stream layout and plans.  0 for DiT / UNetT, whose graphs do not
+           // depend on it (keying them on it would re-capture whenever text lengths differ)
   bool operator==(const GraphKey& o) const {
-    return ws == o.ws && B == o.B && N == o.N && evals == o.evals && packed == o.packed && masked == o.masked;
+    return ws == o.ws && B == o.B && N == o.N && evals == o.evals && packed == o.packed && masked == o.masked &&
+           nt == o.nt;
   }
 };
 struct GraphEntry {
@@ -111,12 +125,19 @@ struct f5_engine {
   f5_arch arch;
   f5_weights w;
   std::vector<f5_layer_weights> layers;
+  std::vector<f5_ctx_layer_weights> ctx;  // MMDiT text stream
   int inner, modW, kin;
   std::mutex mu;
   std::vector<GraphEntry> graphs;
 };
 
-static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int evals, float cfg) {
+static constexpr int kMMDiT = 2;
+
+// MMDiT: first row of block i's modulation vectors in the AdaLN table ([x: 6D | c: 6D] per block, the last block's c
+// part 2D, then norm_out 2D); DiT: [6D] per block, then norm_out
+static size_t mod_block(const f5_arch& A, int i) { return (size_t)i * (A.backbone == kMMDiT ? 12 : 6) * A.dim; }
+
+static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int nt, int evals, float cfg) {
   const f5_arch& A = e->arch;
   Bump bp(ws);
   L.B = B;
@@ -174,6 +195,23 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
     L.cat = bp.take<__half>((size_t)L.M1 * 2 * D);
   }
   L.txu = A.text_avg_upsample ? bp.take<float>((size_t)2 * B * N * Td) : nullptr;
+  L.nt = nt;
+  L.c = L.c0 = nullptr;
+  L.ac = L.qkv_c = L.ao_c = L.g_c = nullptr;
+  L.c_rope_cos = L.c_rope_sin = nullptr;
+  L.c_len = nullptr;
+  if (A.backbone == kMMDiT) {
+    const size_t Mc = (size_t)L.Be * nt;
+    L.c = bp.take<float>(Mc * D);
+    L.c0 = bp.take<float>(Mc * D);
+    L.ac = bp.take<__half>(Mc * D);
+    L.qkv_c = bp.take<__half>(Mc * 3 * e->inner);
+    L.ao_c = bp.take<__half>(Mc * e->inner);
+    L.g_c = bp.take<__half>(Mc * F);
+    L.c_rope_cos = bp.take<float>((size_t)nt * (A.dim_head / 2));
+    L.c_rope_sin = bp.take<float>((size_t)nt * (A.dim_head / 2));
+    L.c_len = bp.take<int>(L.Be);
+  }
   L.bytes = bp.off + 512;
 }
 
@@ -201,6 +239,33 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
     set_error("engine_create: text conv blocks need text_dim %% 64 == 0, <= 512, at most 8 layers");
     return -1;
   }
+  if (arch->backbone < 0 || arch->backbone > kMMDiT) {
+    set_error("engine_create: backbone must be 0 (DiT), 1 (UNetT) or 2 (MMDiT), got %d", arch->backbone);
+    return -1;
+  }
+  if (arch->backbone == kMMDiT) {
+    if (arch->text_dim || arch->conv_layers || arch->long_skip || arch->text_avg_upsample || arch->pe_attn_head >= 0) {
+      set_error("engine_create: MMDiT takes no text_dim, conv_layers, long_skip or text_avg_upsample and applies rope "
+                "to every head (pe_attn_head -1); got text_dim=%d conv_layers=%d long_skip=%d text_avg_upsample=%d "
+                "pe_attn_head=%d", arch->text_dim, arch->conv_layers, arch->long_skip, arch->text_avg_upsample,
+                arch->pe_attn_head);
+      return -1;
+    }
+    if (arch->depth < 1 || weights->ctx_layers == nullptr) {
+      set_error("engine_create: MMDiT needs depth >= 1 and ctx_layers");
+      return -1;
+    }
+    for (int i = 0; i < arch->depth; ++i) {
+      const f5_ctx_layer_weights& c = weights->ctx_layers[i];
+      const bool last = i == arch->depth - 1;
+      if (!c.w_qkv_c || !c.b_qkv_c || (!last && (!c.w_out_c || !c.b_out_c || !c.w_ff1_c || !c.b_ff1_c || !c.w_ff2_c ||
+                                                 !c.b_ff2_c)) ||
+          (arch->qk_norm && (!c.q_norm_c || !c.k_norm_c))) {
+        set_error("engine_create: MMDiT text-stream weights missing in layer %d", i);
+        return -1;
+      }
+    }
+  }
   if ((arch->long_skip || arch->text_avg_upsample) && arch->backbone != 0) {
     set_error("engine_create: long_skip and text_avg_upsample are DiT options");
     return -1;
@@ -222,11 +287,18 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
   if (int rc = configure_kernels()) return rc;
   f5_engine* e = new f5_engine();
   e->arch = *arch;
-  e->w = *weights;
+  // ctx_layers is read only for MMDiT: callers built before it existed pass a struct that ends before it
+  std::memcpy(&e->w, weights, offsetof(f5_weights, ctx_layers));
+  e->w.ctx_layers = nullptr;
   e->layers.assign(weights->layers, weights->layers + arch->depth);
   e->w.layers = e->layers.data();
   e->inner = arch->heads * arch->dim_head;
   e->modW = arch->backbone == 0 ? arch->depth * 6 * arch->dim + 2 * arch->dim : 0;
+  if (arch->backbone == kMMDiT) {
+    e->ctx.assign(weights->ctx_layers, weights->ctx_layers + arch->depth);
+    e->w.ctx_layers = e->ctx.data();
+    e->modW = (int)mod_block(*arch, arch->depth - 1) + 8 * arch->dim + 2 * arch->dim;
+  }
   e->kin = weights->proj_kpad;
   if (e->kin % 64 || e->kin < 2 * arch->mel_dim + arch->text_dim) {
     set_error("engine_create: proj_kpad must be a multiple of 64 covering 2*mel + text_dim");
@@ -242,14 +314,34 @@ void f5_engine_destroy(f5_engine* e) {
   delete e;  // graph holders destroy their executables
 }
 
-size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
+size_t f5_sample_workspace_bytes_nt(const f5_engine* e, int B, int N, int nt, int nfe, float cfg_strength) {
   Layout L;
-  plan_layout(e, L, nullptr, B, N, nfe, cfg_strength);
+  plan_layout(e, L, nullptr, B, N, nt, nfe, cfg_strength);
   return L.bytes;
+}
+
+size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
+  return f5_sample_workspace_bytes_nt(e, B, N, N, nfe, cfg_strength);
+}
+
+double f5_sample_flops_nt(const f5_engine* e, int B, int N, int nt, int nfe, float cfg_strength) {
+  const f5_arch& A = e->arch;
+  if (A.backbone == kMMDiT) {
+    const double D = A.dim, mel = A.mel_dim, F = A.ff_inner, Ld = A.depth, I = e->inner, n = N, m = nt;
+    const double Be = cfg_strength < 1e-5f ? B : 2.0 * B;
+    // every block: audio QKV + out + FF; text QKV; joint attention (QK^T + PV) of the audio queries over N + nt keys.
+    // Every block but the last: text out + FF and the text queries' attention.
+    double per = Ld * (8.0 * n * D * I + 4.0 * n * D * F + 6.0 * m * D * I + 4.0 * n * (n + m) * I) +
+                 (Ld - 1.0) * (2.0 * m * I * D + 4.0 * m * D * F + 4.0 * m * (n + m) * I);
+    per += 2.0 * n * (2 * mel) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n * D * mel;
+    return nfe * Be * per + nfe * (2.0 * 256 * D + 2.0 * D * D + 2.0 * D * (double)e->modW);
+  }
+  return f5_sample_flops(e, B, N, nfe, cfg_strength);
 }
 
 double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
   const f5_arch& A = e->arch;
+  if (A.backbone == kMMDiT) return f5_sample_flops_nt(e, B, N, N, nfe, cfg_strength);
   const double D = A.dim, mel = A.mel_dim, Td = A.text_dim, F = A.ff_inner, Ld = A.depth;
   // attention width heads * dim_head: QKV 6 n D I + out-projection 2 n I D, QK^T + PV 4 n^2 I.  At dim_head 64 the
   // count keeps the form it always had (I = D, as in every shipped config), so figures reported before stay comparable.
@@ -282,7 +374,8 @@ namespace {
 struct StepPlans {
   GemmPlan proj, conv1, conv2, out_proj, long_skip;
   std::vector<GemmPlan> qkv, oproj, ff1, ff2, skip;
-  std::vector<AttnPlan> attn;  // identical per layer, kept once
+  std::vector<GemmPlan> qkv_c, oproj_c, ff1_c, ff2_c;  // MMDiT text stream
+  std::vector<AttnPlan> attn;  // identical per layer, kept once (MMDiT: one with text queries, one for the last block)
 };
 
 #define RC(x)                \
@@ -308,14 +401,82 @@ f5_gemm_args base_args(long long rows, int n_out, int k, int lda, int ldw, int b
 
 constexpr int kAutoTile = 0;  // bn = 0: the GEMM planner picks the tile shape per problem (gemm.cu: pick_tile)
 
+// MMDiT text stream (modules.py:783-846 with context_dim = dim): QKV (+ per-head RMSNorm) + RoPE at text positions
+// 0..nt-1, gated out-projection whose padded rows are zeroed (c_mask, modules.py:700-703), FF pair.  Every text row is
+// computed; the last block has only the QKV.
+int build_text_plans(f5_engine* e, const Layout& L, StepPlans& P) {
+  const f5_arch& A = e->arch;
+  const int D = A.dim, F = A.ff_inner, inner = e->inner;
+  const long long Mc = (long long)L.Be * L.nt;
+  P.qkv_c.resize(A.depth);
+  P.oproj_c.resize(A.depth);
+  P.ff1_c.resize(A.depth);
+  P.ff2_c.resize(A.depth);
+  for (int i = 0; i < A.depth; ++i) {
+    const f5_ctx_layer_weights& cw = e->w.ctx_layers[i];
+    const float* mc = L.mod + mod_block(A, i) + 6 * D;
+    {
+      f5_gemm_args a = base_args(Mc, 3 * inner, D, D, D, kAutoTile, A.qk_norm ? F5_EPI_QKV_NORM_ROPE : F5_EPI_QKV_ROPE,
+                                 F5_ACT_NONE);
+      a.q_norm = cw.q_norm_c;
+      a.k_norm = cw.k_norm_c;
+      a.bias = cw.b_qkv_c;
+      a.out = L.qkv_c;
+      a.ldo = 3 * inner;
+      a.seq = L.nt;
+      a.rope_cos = L.c_rope_cos;
+      a.rope_sin = L.c_rope_sin;
+      a.inner = inner;
+      a.pe_heads = A.heads;
+      a.dim_head = A.dim_head;
+      RC(gemm_plan(&P.qkv_c[i], L.ac, cw.w_qkv_c, &a));
+    }
+    if (i == A.depth - 1) break;  // context_pre_only
+    {
+      f5_gemm_args a = base_args(Mc, D, inner, inner, inner, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
+      a.bias = cw.b_out_c;
+      a.resid = L.c;
+      a.ldo = D;
+      a.seq = L.nt;
+      a.row_len = L.c_len;
+      a.gate = mc + 2 * D;
+      a.step_ptr = L.step_ptr;
+      a.gate_step_stride = e->modW;
+      RC(gemm_plan(&P.oproj_c[i], L.ao_c, cw.w_out_c, &a));
+    }
+    {
+      f5_gemm_args a = base_args(Mc, F, D, D, D, kAutoTile, F5_EPI_F16, F5_ACT_GELU_TANH);
+      a.bias = cw.b_ff1_c;
+      a.out = L.g_c;
+      a.ldo = F;
+      RC(gemm_plan(&P.ff1_c[i], L.ac, cw.w_ff1_c, &a));
+    }
+    {
+      f5_gemm_args a = base_args(Mc, D, F, F, F, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
+      a.bias = cw.b_ff2_c;
+      a.resid = L.c;
+      a.ldo = D;
+      a.gate = mc + 5 * D;
+      a.step_ptr = L.step_ptr;
+      a.gate_step_stride = e->modW;
+      RC(gemm_plan(&P.ff2_c[i], L.g_c, cw.w_ff2_c, &a));
+    }
+  }
+  return 0;
+}
+
 int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, StepPlans& P) {
   const f5_arch& A = e->arch;
   const f5_weights& W = e->w;
   const int D = A.dim, F = A.ff_inner, inner = e->inner;
   const bool dit = A.backbone == 0;
+  const bool mmdit = A.backbone == kMMDiT;
+  const bool adaln = A.backbone != 1;  // DiT and MMDiT: AdaLN modulation from the per-call table
   const bool masked = sa->duration != nullptr;
   const bool strict = masked && sa->exact_varlen;  // every sample exactly as if alone in the batch (f5_sample_args)
-  const bool mask_in = (dit && masked) || strict;  // input projection / conv position embedding see per-sample lengths
+  // input projection / conv position embedding see per-sample lengths (MMDiT's AudioEmbedding takes no mask,
+  // backbones/mmdit.py:67-78: only exact_varlen confines it)
+  const bool mask_in = (dit && masked) || strict;
   const int pe_heads = A.pe_attn_head < 0 ? A.heads : A.pe_attn_head;
   const long long modS = e->modW;
 
@@ -364,7 +525,10 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
   // Variable-length execution (SURVEY.md §8f-1): in the reference's key-masked mode (attn_mask_enabled, modules.py:
   // 513-518) padded rows influence nothing, so every GEMM / conv / attention tile that holds only padding is skipped.
   // In the default "faithful" mode padded keys ARE attended (SURVEY.md §0.5) and every row must be computed.
-  const int skip = (masked && (A.attn_mask_enabled || strict)) ? 1 : 0;
+  const int key_mask = (masked && (A.attn_mask_enabled || strict)) ? 1 : 0;
+  // MMDiT's conv position embedding reads padded audio rows (no mask, mmdit.py:67-78), and those rows evolve with the
+  // ODE like any other: outside exact_varlen they must be computed in full
+  const int skip = mmdit ? (strict ? 1 : 0) : key_mask;
   auto varlen = [&](f5_gemm_args& a) {
     if (!skip) return;
     a.row_len = L.row_len;
@@ -403,8 +567,8 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
       a.ldo = D;
       a.seq = L.seq;
       a.row_len = rl;
-      if (dit) {
-        a.gate = L.mod + (size_t)i * 6 * D + 2 * D;
+      if (adaln) {
+        a.gate = L.mod + mod_block(A, i) + 2 * D;
         a.step_ptr = L.step_ptr;
         a.gate_step_stride = modS;
       }
@@ -424,8 +588,8 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
       a.bias = lw.b_ff2;
       a.resid = L.x;
       a.ldo = D;
-      if (dit) {
-        a.gate = L.mod + (size_t)i * 6 * D + 5 * D;
+      if (adaln) {
+        a.gate = L.mod + mod_block(A, i) + 5 * D;
         a.step_ptr = L.step_ptr;
         a.gate_step_stride = modS;
       }
@@ -447,7 +611,17 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
     RC(gemm_plan(&P.out_proj, L.a, W.out_w, &a));
   }
   P.attn.resize(1);
-  RC(attn_plan(&P.attn[0], L.qkv, L.ao, L.Be, L.seq, A.heads, A.dim_head, skip ? L.kv_len : nullptr,
+  if (mmdit) {
+    RC(build_text_plans(e, L, P));
+    // joint attention: [0] for the blocks with text queries, [1] for the last block, whose text output is discarded
+    P.attn.resize(2);
+    for (int last = 0; last < 2; ++last)
+      RC(attn_joint_plan(&P.attn[last], L.qkv, L.qkv_c, L.ao, L.ao_c, L.Be, L.seq, L.nt, A.heads, A.dim_head,
+                         key_mask ? L.kv_len : nullptr, key_mask ? L.c_len : nullptr, last ? 0 : 1,
+                         1.0f / sqrtf((float)A.dim_head)));
+    return 0;
+  }
+  RC(attn_plan(&P.attn[0], L.qkv, L.ao, L.Be, L.seq, A.heads, A.dim_head, key_mask ? L.kv_len : nullptr,
                1.0f / sqrtf((float)A.dim_head)));
   return 0;
 }
@@ -464,10 +638,10 @@ static constexpr bool diag_skip(const char*) { return false; }
 #endif
 
 int norm_mod(const f5_engine* e, const Layout& L, const float* x, long long rows, int mode, const float* a,
-             const float* b, bool step_indexed, cudaStream_t s) {
+             const float* b, bool step_indexed, cudaStream_t s, __half* out = nullptr) {
   NormParams p{};
   p.x = x;
-  p.out = L.a;
+  p.out = out ? out : L.a;
   p.rows = (int)rows;
   p.D = e->arch.dim;
   p.eps = 1e-6f;
@@ -480,21 +654,59 @@ int norm_mod(const f5_engine* e, const Layout& L, const float* x, long long rows
   return run_row_norm(mode, p, s);
 }
 
+// One MMDiT block (modules.py:806-846): both streams' AdaLN, QKV, joint attention, gated out-projections and FF pairs
+int run_mmdit_block(f5_engine* e, const Layout& L, const StepPlans& P, int i, cudaStream_t s) {
+  const f5_arch& A = e->arch;
+  const int D = A.dim;
+  const bool last = i == A.depth - 1;
+  const long long Mc = (long long)L.Be * L.nt;
+  const float* mx = L.mod + mod_block(A, i);
+  const float* mc = mx + 6 * D;
+  RC(norm_mod(e, L, L.x, L.M1, 0, mx + D, mx, true, s));  // attn_norm_x: scale_msa, shift_msa
+  if (last)
+    RC(norm_mod(e, L, L.c, Mc, 0, mc, mc + D, true, s, L.ac));  // AdaLayerNorm_Final: scale, shift
+  else
+    RC(norm_mod(e, L, L.c, Mc, 0, mc + D, mc, true, s, L.ac));
+  RC(gemm_run(P.qkv[i], s));
+  RC(gemm_run(P.qkv_c[i], s));
+  RC(attn_run(P.attn[last ? 1 : 0], s));
+  RC(gemm_run(P.oproj[i], s));
+  if (!last) {
+    RC(gemm_run(P.oproj_c[i], s));
+    RC(norm_mod(e, L, L.c, Mc, 0, mc + 4 * D, mc + 3 * D, true, s, L.ac));  // ff_norm_c: c_scale_mlp, c_shift_mlp
+    RC(gemm_run(P.ff1_c[i], s));
+    RC(gemm_run(P.ff2_c[i], s));
+  }
+  RC(norm_mod(e, L, L.x, L.M1, 0, mx + 4 * D, mx + 3 * D, true, s));  // ff_norm_x: scale_mlp, shift_mlp
+  RC(gemm_run(P.ff1[i], s));
+  return gemm_run(P.ff2[i], s);
+}
+
 int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const StepPlans& P, cudaStream_t s) {
   const f5_arch& A = e->arch;
   const int D = A.dim;
   const bool dit = A.backbone == 0;
+  const bool mmdit = A.backbone == kMMDiT;
   RC(gemm_run(P.proj, s));
   if (!diag_skip("conv")) {
     RC(gemm_run(P.conv1, s));
     RC(gemm_run(P.conv2, s));
   }
-  if (!dit) RC(run_prepend_time_token(L.x, L.h0, L.temb, L.step_ptr, L.N, D, L.M1, s));
+  if (A.backbone == 1) RC(run_prepend_time_token(L.x, L.h0, L.temb, L.step_ptr, L.N, D, L.M1, s));
+  if (mmdit) {
+    // the text stream restarts from its embedding at every evaluation (get_input_embed, mmdit.py:177-196)
+    RC(check_cuda(cudaMemcpyAsync(L.c, L.c0, sizeof(float) * L.Be * L.nt * D,
+                                  cudaMemcpyDeviceToDevice, s), "text stream copy"));
+  }
   if (A.long_skip)
     RC(check_cuda(cudaMemcpyAsync(L.x_embed, L.x, sizeof(float) * L.M1 * D, cudaMemcpyDeviceToDevice, s),
                   "long skip copy"));
   const int half = A.depth / 2;
   for (int i = 0; i < A.depth; ++i) {
+    if (mmdit) {
+      RC(run_mmdit_block(e, L, P, i, s));
+      continue;
+    }
     const f5_layer_weights& lw = e->w.layers[i];
     if (dit) {
       const float* m = L.mod + (size_t)i * 6 * D;
@@ -525,8 +737,8 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
     RC(run_concat_half(L.x, L.x_embed, L.cat, L.M1, D, s));
     RC(gemm_run(P.long_skip, s));
   }
-  if (dit) {
-    const float* m = L.mod + (size_t)A.depth * 6 * D;
+  if (dit || mmdit) {
+    const float* m = L.mod + (e->modW - 2 * D);
     RC(norm_mod(e, L, L.x, L.M1, 0, m, m + D, true, s));  // AdaLayerNorm_Final: scale, shift (modules.py:342-347)
   } else {
     RC(norm_mod(e, L, L.x, L.M1, 2, e->w.g_out, nullptr, false, s));
@@ -544,7 +756,7 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
   ep.packed = L.packed;
   ep.N = L.N;
   ep.seq_tok = L.seq;
-  ep.tok_off = dit ? 0 : 1;
+  ep.tok_off = A.backbone == 1 ? 1 : 0;
   ep.B = L.B;
   return run_cfg_euler(ep, s);
 }
@@ -554,6 +766,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   const f5_weights& W = e->w;
   const int D = A.dim, Td = A.text_dim, B = L.B, N = L.N, S = L.evals;
   const bool dit = A.backbone == 0;
+  const bool mmdit = A.backbone == kMMDiT;
   const bool masked = sa->duration != nullptr;
   const bool strict = masked && sa->exact_varlen;
   // small host -> device control data (pageable source: cudaMemcpyAsync stages it before returning).
@@ -588,7 +801,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     RC(check_cuda(cudaMemcpyAsync(hd.data(), sa->duration, sizeof(int) * B, cudaMemcpyDeviceToHost, s), "dur d2h"));
     RC(check_cuda(cudaStreamSynchronize(s), "dur sync"));
     std::vector<int> rl(L.Be);
-    for (int i = 0; i < L.Be; ++i) rl[i] = hd[i % B] + (dit ? 0 : 1);
+    for (int i = 0; i < L.Be; ++i) rl[i] = hd[i % B] + (A.backbone == 1 ? 1 : 0);
     RC(check_cuda(cudaMemcpyAsync(L.row_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "row_len"));
     RC(check_cuda(cudaMemcpyAsync(L.kv_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "kv_len"));
     RC(check_cuda(cudaMemcpyAsync(L.valid_len, hd.data(), sizeof(int) * B, cudaMemcpyHostToDevice, s), "valid_len"));
@@ -609,7 +822,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   RC(run_time_features(L.t_dev, L.tfeat, S, 256, s));
   RC(run_small_linear(1, L.tfeat, reinterpret_cast<const __half*>(W.time_w0), W.time_b0, L.th1, S, 256, D, s));
   RC(run_small_linear(0, L.th1, reinterpret_cast<const __half*>(W.time_w1), W.time_b1, L.temb, S, D, D, s));
-  if (dit) {
+  if (dit || mmdit) {
     RC(run_silu_to_half(L.temb, L.temb_silu, (long long)S * D, s));
     f5_gemm_args a = base_args(S, e->modW, D, D, D, 128, F5_EPI_F32, F5_ACT_NONE);
     a.bias = W.mod_b;
@@ -618,6 +831,11 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     GemmPlan pl;
     RC(gemm_plan(&pl, L.temb_silu, W.mod_w, &a));
     RC(gemm_run(pl, s));
+  }
+  if (mmdit) {  // text embedding of both CFG variants and the text rope table; no text columns in the input projection
+    RC(run_mmdit_text_embed(sa->text, B, L.Be, L.nt, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding, L.c0,
+                            L.c_len, s));
+    RC(run_rope_table(L.c_rope_cos, L.c_rope_sin, L.nt, A.dim_head / 2, s));
   }
   // text embedding, both CFG variants (dit.py:86-139 / unett.py:55-84)
   TextGatherParams tp{};
@@ -632,7 +850,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   tp.add_pos = A.conv_layers > 0;
   tp.out = L.tx;
   tp.filler = L.filler;
-  RC(run_text_gather(tp, s));
+  if (!mmdit) RC(run_text_gather(tp, s));
   const int R2 = 2 * B * N;
   for (int i = 0; i < A.conv_layers; ++i) {
     if (A.text_mask_padding) RC(run_mask_rows(L.tx, L.filler, B * N, R2, Td, s));
@@ -688,7 +906,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
 int copy_v_out(const f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaStream_t s) {
   if (!sa->v_out) return 0;
   const int mel = e->arch.mel_dim;
-  const int off = e->arch.backbone == 0 ? 0 : 1;
+  const int off = e->arch.backbone == 1 ? 1 : 0;
   for (int b = 0; b < L.Be; ++b)
     RC(check_cuda(cudaMemcpyAsync(sa->v_out + (size_t)b * L.N * mel, L.v + ((size_t)b * L.seq + off) * mel,
                                   sizeof(float) * L.N * mel, cudaMemcpyDeviceToDevice, s),
@@ -714,7 +932,7 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
   }
   const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
   Layout L;
-  plan_layout(e, L, workspace, sa->B, sa->N, evals, sa->cfg_strength);
+  plan_layout(e, L, workspace, sa->B, sa->N, sa->nt, evals, sa->cfg_strength);
   if (ws_bytes < L.bytes) {
     set_error("f5_sample: workspace too small (%zu < %zu)", ws_bytes, L.bytes);
     return -1;
@@ -722,7 +940,7 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
   RC(run_prologue(e, L, sa, s));
   if (sa->use_graph) {
     const GraphKey key{workspace, sa->B, sa->N, evals, L.packed,
-                       sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1)};
+                       sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1), e->arch.backbone == kMMDiT ? sa->nt : 0};
     std::shared_ptr<GraphHolder> g;
     {
       std::lock_guard<std::mutex> lk(e->mu);

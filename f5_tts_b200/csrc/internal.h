@@ -49,9 +49,18 @@ struct AttnPlan {
   AttnParams p;
   dim3 grid;
   int dh;  // head width: 64 or 128
+  // joint (MMDiT) attention: text segment
+  int joint = 0;
+  CUtensorMap tmC;
+  AttnJointParams jp;
 };
 int attn_plan(AttnPlan* plan, const void* qkv, void* out, int batches, int seq, int heads, int dim_head,
               const int* kv_len, float scale);
+// Joint attention over [audio | text] keys for [audio | text] queries.  qkv_c fp16 [batches*seq_c, 3*inner], out_c
+// [batches*seq_c, inner]; c_len [batches] valid text keys (0 allowed) or null; text_q = 0 computes the audio queries
+// only (out_c is not written).
+int attn_joint_plan(AttnPlan* plan, const void* qkv, const void* qkv_c, void* out, void* out_c, int batches, int seq,
+                    int seq_c, int heads, int dim_head, const int* kv_len, const int* c_len, int text_q, float scale);
 int attn_run(const AttnPlan& plan, cudaStream_t s);
 
 // fp16 tensor map of rank 2 to 4, 128B swizzle: dims[0] is contiguous, strides[i] is the byte stride of dims[i + 1],
@@ -67,6 +76,9 @@ namespace f5 {
 int run_row_norm(int mode, const NormParams& p, cudaStream_t s);
 int run_dwconv7_ln(const DwConvLnParams& p, cudaStream_t s);
 int run_text_gather(const TextGatherParams& p, cudaStream_t s);
+// MMDiT text embedding of Be = B (cond) or 2B (cond, uncond) variants: out fp32 [Be*nt, D], c_len [Be]
+int run_mmdit_text_embed(const long long* ids, int B, int Be, int nt, int D, const float* table, int num_embeds,
+                         int mask_padding, float* out, int* c_len, cudaStream_t s);
 // text_embedding_average_upsampling: tx -> out, both fp32 [2B, N, Td]; valid_len [B] audio lengths or null (= N)
 int run_text_avg_upsample(const float* tx, float* out, const uint8_t* filler, const int* valid_len, int B, int N,
                           int nt, int Td, cudaStream_t s);

@@ -66,6 +66,14 @@ struct AttnParams {
   __half* out;        // [Be*seq, inner]
 };
 
+// Second key / query segment of the joint (MMDiT) attention kernel
+struct AttnJointParams {
+  int seq_c;          // text tokens per sample
+  const int* c_len;   // [Be] valid text keys per sample (0 allowed), or null (= seq_c)
+  __half* out_c;      // [Be*seq_c, inner]
+  int q_blocks_a;     // audio query blocks, ceil(seq / kAttnBQ); grid.x beyond them are text query blocks
+};
+
 constexpr int kAttnThreads = 288;   // two softmax / MMA warpgroups (64 query rows each) + one TMA producer warp
 constexpr int kAttnBQ = 128;        // query rows per CTA
 constexpr int kAttnBKV = 128;       // keys per tile

@@ -83,6 +83,13 @@ int run_text_gather(const TextGatherParams& p, cudaStream_t s) {
   return check_launch("text_gather_kernel");
 }
 
+int run_mmdit_text_embed(const long long* ids, int B, int Be, int nt, int D, const float* table, int num_embeds,
+                         int mask_padding, float* out, int* c_len, cudaStream_t s) {
+  mmdit_text_embed_kernel<<<Be * nt, 128, 0, s>>>(ids, B, nt, D, table, num_embeds, mask_padding, out, c_len);
+  count_launch();
+  return check_launch("mmdit_text_embed_kernel");
+}
+
 int run_text_avg_upsample(const float* tx, float* out, const uint8_t* filler, const int* valid_len, int B, int N,
                           int nt, int Td, cudaStream_t s) {
   const int K = nt < N ? nt : N;

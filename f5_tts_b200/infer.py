@@ -16,7 +16,7 @@ import wave
 import numpy as np
 import torch
 
-from .model import CFM, DiT, UNetT  # noqa: F401
+from .model import CFM, DiT, MMDiT, UNetT  # noqa: F401
 from . import vocoder as _vocoder
 from .vocoder import Vocos
 

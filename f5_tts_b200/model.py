@@ -9,6 +9,7 @@ Reference anchors (relative to /root/reference/src/f5_tts):
   CFM.sample            model/cfm.py:83-229
   DiT                   model/backbones/dit.py:170-370      (forward 319-370)
   UNetT                 model/backbones/unett.py:108-307    (forward 244-307)
+  MMDiT                 model/backbones/mmdit.py:85-246     (forward 198-246)
   MelSpec               model/modules.py:112-151
   lens_to_mask etc.     model/utils.py:53-58, 88-106, 205-218
 """
@@ -93,9 +94,51 @@ def _attach(root: nn.Module, dotted: str, tensor: torch.Tensor, buffer=False):
         mod.register_parameter(leaf, nn.Parameter(tensor, requires_grad=False))
 
 
+def _mmdit_spec(*, dim, depth, heads, dim_head, ff_mult, mel_dim, text_num_embeds, qk_norm=None):
+    """(key, shape, init) of every tensor of backbones/mmdit.py's MMDiT, in its registration order."""
+    D, inner, ff = dim, heads * dim_head, int(dim * ff_mult)
+    out = []
+
+    def lin(p, o, i, init="w"):
+        out.extend([(p + ".weight", (o, i), init), (p + ".bias", (o,), "zero")])
+
+    lin("time_embed.time_mlp.0", D, 256)
+    lin("time_embed.time_mlp.2", D, D)
+    out.append(("text_embed.text_embed.weight", (text_num_embeds + 1, D), "w"))
+    lin("audio_embed.linear", D, 2 * mel_dim)
+    for i in (0, 2):
+        out += [(f"audio_embed.conv_pos_embed.conv1d.{i}.weight", (D, D // 16, 31), "w"),
+                (f"audio_embed.conv_pos_embed.conv1d.{i}.bias", (D,), "zero")]
+    for i in range(depth):
+        b, last = f"transformer_blocks.{i}.", i == depth - 1  # the last block is context_pre_only (modules.py:781)
+        lin(b + "attn_norm_c.linear", (2 if last else 6) * D, D, init="zero")  # AdaLN-Zero (mmdit.py:150-156)
+        lin(b + "attn_norm_x.linear", 6 * D, D, init="zero")
+        for nm in ("to_q", "to_k", "to_v"):
+            lin(b + "attn." + nm, inner, D)
+        if qk_norm is not None:
+            out += [(b + "attn.q_norm.weight", (dim_head,), "one"), (b + "attn.k_norm.weight", (dim_head,), "one")]
+        for nm in ("to_q_c", "to_k_c", "to_v_c"):
+            lin(b + "attn." + nm, inner, D)
+        if qk_norm is not None:
+            out += [(b + "attn.c_q_norm.weight", (dim_head,), "one"), (b + "attn.c_k_norm.weight", (dim_head,), "one")]
+        lin(b + "attn.to_out.0", D, inner)
+        if not last:
+            lin(b + "attn.to_out_c", D, inner)
+            lin(b + "ff_c.ff.0.0", ff, D)
+            lin(b + "ff_c.ff.2", D, ff)
+        lin(b + "ff_x.ff.0.0", ff, D)
+        lin(b + "ff_x.ff.2", D, ff)
+    lin("norm_out.linear", 2 * D, D, init="zero")
+    lin("proj_out", mel_dim, D, init="zero")
+    return out
+
+
 def _backbone_spec(kind: str, *, dim, depth, heads, dim_head, ff_mult, mel_dim, text_num_embeds, text_dim,
                    conv_layers, qk_norm=None, long_skip_connection=False):
-    """(key, shape, init) for every tensor of the backbone; identical names to dit.py / unett.py modules."""
+    """(key, shape, init) for every tensor of the backbone; identical names to dit.py / unett.py / mmdit.py modules."""
+    if kind == "MMDiT":
+        return _mmdit_spec(dim=dim, depth=depth, heads=heads, dim_head=dim_head, ff_mult=ff_mult, mel_dim=mel_dim,
+                           text_num_embeds=text_num_embeds, qk_norm=qk_norm)
     D, T, Mel = dim, text_dim, mel_dim
     inner, ff = heads * dim_head, int(dim * ff_mult)
     out = []
@@ -291,12 +334,13 @@ class _Backbone(nn.Module):
         steps = len(t_grid) - 1
         assert y.is_contiguous() and step_cond.is_contiguous() and text.is_contiguous()
         assert y.dtype == torch.float32 and step_cond.dtype == torch.float32 and text.dtype == torch.int64
-        need = L.f5_sample_workspace_bytes(st["handle"], B, N, _nfe(steps, method), float(cfg_strength))
+        nt = text.shape[1]
+        need = L.f5_sample_workspace_bytes_nt(st["handle"], B, N, nt, _nfe(steps, method), float(cfg_strength))
         stream = torch.cuda.current_stream(y.device).cuda_stream
         ws = self._ws_acquire(need, y.device, stream)
         tg = (C.c_float * (steps + 1))(*[float(v) for v in t_grid])
         a = _lib.SampleArgs()
-        a.B, a.N, a.nt, a.steps = B, N, text.shape[1], steps
+        a.B, a.N, a.nt, a.steps = B, N, nt, steps
         a.text, a.step_cond, a.y = text.data_ptr(), step_cond.data_ptr(), y.data_ptr()
         a.duration = duration.data_ptr() if duration is not None else None
         a.t = tg
@@ -312,9 +356,10 @@ class _Backbone(nn.Module):
         finally:
             self._ws_release(ws, y.device, stream)
 
-    def sample_flops(self, B, N, steps, cfg_strength, method="euler") -> float:
-        return float(_lib.lib().f5_sample_flops(self.engine()["handle"], B, N, _nfe(steps, method),
-                                                float(cfg_strength)))
+    def sample_flops(self, B, N, steps, cfg_strength, method="euler", nt=None) -> float:
+        """Algorithmic FLOPs of one run(); nt (text length) matters for MMDiT only, None counts nt = N."""
+        return float(_lib.lib().f5_sample_flops_nt(self.engine()["handle"], B, N, N if nt is None else nt,
+                                                   _nfe(steps, method), float(cfg_strength)))
 
     # -- the reference's operator signature (dit.py:319-330 / unett.py:244-255) ----------------------------------
     @torch.no_grad()
@@ -348,6 +393,22 @@ class UNetT(_Backbone):
     """backbones/unett.py:108-128"""
 
     KIND = "UNetT"
+
+
+class MMDiT(_Backbone):
+    """backbones/mmdit.py:85-121: joint audio-text attention over two residual streams (the text is not padded to the
+    audio length).  Same constructor arguments as the reference; checkpoint_activations (training only) is accepted and
+    ignored, attn_backend is accepted for config compatibility."""
+
+    KIND = "MMDiT"
+
+    def __init__(self, *, dim, depth=8, heads=8, dim_head=64, dropout=0.1, ff_mult=4, mel_dim=100, text_num_embeds=256,
+                 text_mask_padding=True, qk_norm=None, checkpoint_activations=False, attn_backend="torch",
+                 attn_mask_enabled=False):
+        super().__init__(dim=dim, depth=depth, heads=heads, dim_head=dim_head, dropout=dropout, ff_mult=ff_mult,
+                         mel_dim=mel_dim, text_num_embeds=text_num_embeds, text_dim=0,
+                         text_mask_padding=text_mask_padding, qk_norm=qk_norm, conv_layers=0, pe_attn_head=None,
+                         attn_backend=attn_backend, attn_mask_enabled=attn_mask_enabled)
 
 
 # ----------------------------------------------------------------------------------------------------------------

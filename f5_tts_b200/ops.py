@@ -128,6 +128,25 @@ def attention(qkv: torch.Tensor, batches: int, seq: int, heads: int, kv_len=None
     return out
 
 
+def attention_joint(qkv: torch.Tensor, qkv_c: torch.Tensor, batches: int, seq: int, seq_c: int, heads: int,
+                    kv_len=None, c_len=None, text_q=True, scale=None, dim_head=64):
+    """MMDiT joint attention: queries [audio | text] over keys [audio | text].  qkv fp16 [batches*seq, 3*inner], qkv_c
+    fp16 [batches*seq_c, 3*inner] -> (out [batches*seq, inner], out_c [batches*seq_c, inner]); kv_len / c_len int32
+    [batches] valid audio / text keys or None; text_q=False leaves out_c unwritten (torch.empty)."""
+    _need_cuda(qkv, qkv_c, kv_len, c_len)
+    inner = heads * dim_head
+    assert qkv.dtype == torch.float16 and qkv.is_contiguous() and qkv.shape == (batches * seq, 3 * inner)
+    assert qkv_c.dtype == torch.float16 and qkv_c.is_contiguous() and qkv_c.shape == (batches * seq_c, 3 * inner)
+    out = torch.empty((batches * seq, inner), dtype=torch.float16, device=qkv.device)
+    out_c = torch.empty((batches * seq_c, inner), dtype=torch.float16, device=qkv.device)
+    scale = dim_head ** -0.5 if scale is None else scale
+    with torch.cuda.device(qkv.device):
+        _lib.check(_lib.lib().f5_attention_joint(qkv.data_ptr(), qkv_c.data_ptr(), out.data_ptr(), out_c.data_ptr(),
+                                                 batches, seq, seq_c, heads, dim_head, _ptr(kv_len), _ptr(c_len),
+                                                 1 if text_q else 0, scale, _stream(qkv)), "f5_attention_joint")
+    return out, out_c
+
+
 def row_norm(x: torch.Tensor, mode: int, a: torch.Tensor, b: Optional[torch.Tensor] = None, eps=1e-6) -> torch.Tensor:
     _need_cuda(x, a, b)
     assert x.dtype == torch.float32 and x.is_contiguous()

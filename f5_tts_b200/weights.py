@@ -7,7 +7,10 @@
  * input_embed.proj K padded with zero columns to a multiple of 64;
  * grouped Conv1d(k=31, g=16) weight [D, G, 31] -> [31][D][G], G = D/16 channels per group, so that tap t / group g
    is a K-major G x G block (64 x 64 at D = 1024);
- * biases, norm gains, GRN parameters, embedding table -> fp32.
+ * biases, norm gains, GRN parameters, embedding table -> fp32;
+ * MMDiT: the audio stream fills the per-layer slots of DiT (audio_embed.linear is the input projection, its K = 2*mel
+   zero-padded to 256), the text stream goes to `C{i}.*` (to_q_c|to_k_c|to_v_c stacked), and the AdaLN table is
+   [attn_norm_x 6D | attn_norm_c 6D (2D in the last block)] per block, then norm_out.
 The packed tensors are owned by Python (kept alive in the returned dict); the C engine only stores pointers.
 """
 from __future__ import annotations
@@ -35,6 +38,8 @@ def packed_tensors(m) -> dict[str, torch.Tensor]:
     if dev.type != "cuda":
         raise _lib.F5LibraryError("the backbone must live on a CUDA (H100) device before sampling; no CPU path exists")
     D, depth = m.dim, m.depth
+    if m.KIND == "MMDiT":
+        return _packed_mmdit(m, sd, dev)
     dit = m.KIND == "DiT"
     T: dict[str, torch.Tensor] = {}
     T["time_w0"], T["time_b0"] = _h(sd["time_embed.time_mlp.0.weight"]), _f(sd["time_embed.time_mlp.0.bias"])
@@ -86,11 +91,53 @@ def packed_tensors(m) -> dict[str, torch.Tensor]:
     return T
 
 
+def _packed_mmdit(m, sd, dev) -> dict[str, torch.Tensor]:
+    D, depth = m.dim, m.depth
+    T: dict[str, torch.Tensor] = {}
+    T["time_w0"], T["time_b0"] = _h(sd["time_embed.time_mlp.0.weight"]), _f(sd["time_embed.time_mlp.0.bias"])
+    T["time_w1"], T["time_b1"] = _h(sd["time_embed.time_mlp.2.weight"]), _f(sd["time_embed.time_mlp.2.bias"])
+    T["text_table"] = _f(sd["text_embed.text_embed.weight"])
+    pw = sd["audio_embed.linear.weight"]
+    kin = pw.shape[1]
+    kpad = (kin + 63) // 64 * 64
+    pwp = torch.zeros((D, kpad), dtype=torch.float16, device=dev)
+    pwp[:, :kin] = pw.to(torch.float16)
+    T["proj_w"], T["proj_b"] = pwp, _f(sd["audio_embed.linear.bias"])
+    for j, idx in enumerate((0, 2)):
+        cw = sd[f"audio_embed.conv_pos_embed.conv1d.{idx}.weight"]
+        T[f"conv_w{j}"] = _h(cw.permute(2, 0, 1))
+        T[f"conv_b{j}"] = _f(sd[f"audio_embed.conv_pos_embed.conv1d.{idx}.bias"])
+    mw, mb = [], []
+    for i in range(depth):
+        p, a, q, c = f"transformer_blocks.{i}.", f"transformer_blocks.{i}.attn.", f"L{i}.", f"C{i}."
+        T[q + "w_qkv"] = _h(torch.cat([sd[a + "to_q.weight"], sd[a + "to_k.weight"], sd[a + "to_v.weight"]], dim=0))
+        T[q + "b_qkv"] = _f(torch.cat([sd[a + "to_q.bias"], sd[a + "to_k.bias"], sd[a + "to_v.bias"]], dim=0))
+        T[q + "w_out"], T[q + "b_out"] = _h(sd[a + "to_out.0.weight"]), _f(sd[a + "to_out.0.bias"])
+        T[q + "w_ff1"], T[q + "b_ff1"] = _h(sd[p + "ff_x.ff.0.0.weight"]), _f(sd[p + "ff_x.ff.0.0.bias"])
+        T[q + "w_ff2"], T[q + "b_ff2"] = _h(sd[p + "ff_x.ff.2.weight"]), _f(sd[p + "ff_x.ff.2.bias"])
+        T[c + "w_qkv_c"] = _h(torch.cat([sd[a + "to_q_c.weight"], sd[a + "to_k_c.weight"], sd[a + "to_v_c.weight"]], 0))
+        T[c + "b_qkv_c"] = _f(torch.cat([sd[a + "to_q_c.bias"], sd[a + "to_k_c.bias"], sd[a + "to_v_c.bias"]], 0))
+        if i < depth - 1:
+            T[c + "w_out_c"], T[c + "b_out_c"] = _h(sd[a + "to_out_c.weight"]), _f(sd[a + "to_out_c.bias"])
+            T[c + "w_ff1_c"], T[c + "b_ff1_c"] = _h(sd[p + "ff_c.ff.0.0.weight"]), _f(sd[p + "ff_c.ff.0.0.bias"])
+            T[c + "w_ff2_c"], T[c + "b_ff2_c"] = _h(sd[p + "ff_c.ff.2.weight"]), _f(sd[p + "ff_c.ff.2.bias"])
+        if m.qk_norm is not None:
+            T[q + "q_norm_w"], T[q + "k_norm_w"] = _f(sd[a + "q_norm.weight"]), _f(sd[a + "k_norm.weight"])
+            T[c + "q_norm_c"], T[c + "k_norm_c"] = _f(sd[a + "c_q_norm.weight"]), _f(sd[a + "c_k_norm.weight"])
+        mw += [sd[p + "attn_norm_x.linear.weight"], sd[p + "attn_norm_c.linear.weight"]]
+        mb += [sd[p + "attn_norm_x.linear.bias"], sd[p + "attn_norm_c.linear.bias"]]
+    mw.append(sd["norm_out.linear.weight"])
+    mb.append(sd["norm_out.linear.bias"])
+    T["mod_w"], T["mod_b"] = _h(torch.cat(mw, dim=0)), _f(torch.cat(mb, dim=0))
+    T["out_w"], T["out_b"] = _h(sd["proj_out.weight"]), _f(sd["proj_out.bias"])
+    return T
+
+
 def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
     """Create the C engine over already-packed tensors (fresh from `packed_tensors` or read back from the disk cache)."""
     dev = next(iter(T.values())).device
     depth = m.depth
-    dit = m.KIND == "DiT"
+    dit = m.KIND != "UNetT"  # DiT and MMDiT: AdaLN table
     P = lambda k: T[k].data_ptr() if k in T else None  # noqa: E731
     W = _lib.Weights()
     W.time_w0, W.time_b0, W.time_w1, W.time_b1 = P("time_w0"), P("time_b0"), P("time_w1"), P("time_b1")
@@ -115,9 +162,17 @@ def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
         W.g_out = P("g_out")
     W.out_w, W.out_b = P("out_w"), P("out_b")
     W.long_skip_w = P("long_skip_w")
+    ctx = None
+    if m.KIND == "MMDiT":
+        ctx = (_lib.CtxLayerWeights * depth)()
+        for i in range(depth):
+            for name in ("w_qkv_c", "b_qkv_c", "w_out_c", "b_out_c", "w_ff1_c", "b_ff1_c", "w_ff2_c", "b_ff2_c",
+                         "q_norm_c", "k_norm_c"):
+                setattr(ctx[i], name, P(f"C{i}." + name))
+        W.ctx_layers = C.cast(ctx, C.POINTER(_lib.CtxLayerWeights))
 
     A = _lib.Arch()
-    A.backbone = 0 if dit else 1
+    A.backbone = _lib.BACKBONES[m.KIND]
     A.dim, A.depth, A.heads, A.dim_head, A.ff_inner = m.dim, depth, m.heads, m.dim_head, m.ff_inner
     A.mel_dim, A.text_dim, A.text_num_embeds, A.conv_layers = m.mel_dim, m.text_dim, m.text_num_embeds, m.conv_layers
     A.text_mask_padding = 1 if m.text_mask_padding else 0
@@ -129,7 +184,7 @@ def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
     handle = C.c_void_p()
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().f5_engine_create(C.byref(A), C.byref(W), C.byref(handle)), "f5_engine_create")
-    return {"handle": handle, "keep": T, "layers": layers, "weights": W, "arch": A}
+    return {"handle": handle, "keep": T, "layers": layers, "ctx": ctx, "weights": W, "arch": A}
 
 
 def pack_backbone(m) -> dict:

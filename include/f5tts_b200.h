@@ -97,6 +97,17 @@ int f5_attention(const void* qkv, void* out, int batches, int seq, int heads, co
 int f5_attention_dh(const void* qkv, void* out, int batches, int seq, int heads, int dim_head, const int* kv_len,
                     float scale, f5_stream_t stream);
 
+/* Joint attention of MMDiT (model/modules.py:563-705, JointAttnProcessor): one softmax over the keys [audio | text]
+ * for the queries [audio | text].  The two segments are separate fused QKV buffers:
+ *   qkv   fp16 [batches*seq,   3*heads*dim_head]   out   fp16 [batches*seq,   heads*dim_head]
+ *   qkv_c fp16 [batches*seq_c, 3*heads*dim_head]   out_c fp16 [batches*seq_c, heads*dim_head]
+ * kv_len [batches] valid audio keys (>= 1) or NULL (= seq); c_len [batches] valid text keys (0 = the text segment adds no
+ * key) or NULL (= seq_c); both device int32.  text_q = 0 computes the audio queries only and leaves out_c unwritten
+ * (the last MMDiT block discards its text output).  dim_head 64 or 128.  Since f5_version() 107. */
+int f5_attention_joint(const void* qkv, const void* qkv_c, void* out, void* out_c, int batches, int seq, int seq_c,
+                       int heads, int dim_head, const int* kv_len, const int* c_len, int text_q, float scale,
+                       f5_stream_t stream);
+
 /* Row normalisation + modulation -> fp16 (model/modules.py:312-326,333-347,753; x_transformers RMSNorm unett.py:154)
  *   mode 0: LN(eps) * (1 + a[c]) + b[c]   mode 1: LN(eps) * a[c] + b[c]   mode 2: x/||x|| * sqrt(D) * a[c] */
 int f5_row_norm(const float* x, void* out_f16, int rows, int D, int mode, float eps, const float* a, const float* b,
@@ -135,11 +146,13 @@ int f5_vocos_decode_varlen(const f5_vocos_weights* w, const float* mel, int B, i
                            void* workspace, size_t ws_bytes, float* wav, f5_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
- * Engine: the whole CFM.sample NFE loop (model/cfm.py:160-223) for a DiT (backbones/dit.py:319-370) or UNetT
- * (backbones/unett.py:244-307) backbone.
+ * Engine: the whole CFM.sample NFE loop (model/cfm.py:160-223) for a DiT (backbones/dit.py:319-370), UNetT
+ * (backbones/unett.py:244-307) or MMDiT (backbones/mmdit.py:198-246) backbone.
  * ------------------------------------------------------------------------------------------------------------ */
 typedef struct {
-  int backbone;          /* 0 = DiT, 1 = UNetT */
+  /* 0 = DiT, 1 = UNetT, 2 = MMDiT (since f5_version() 107).  MMDiT needs text_dim = conv_layers = long_skip =
+   * text_avg_upsample = 0 and pe_attn_head = -1 (rope on every head), and f5_weights.ctx_layers. */
+  int backbone;
   /* dim_head: 64, or since f5_version() 106 also 128 (rope over the full head, softmax scale 1/sqrt(dim_head));
    * heads * dim_head must be a multiple of 128 and at most 1024 at dim_head 128 */
   int dim, depth, heads, dim_head, ff_inner, mel_dim, text_dim, text_num_embeds, conv_layers;
@@ -166,6 +179,16 @@ typedef struct {
                                                    (modules.py:406-407), else NULL */
 } f5_layer_weights;
 
+/* MMDiT text-stream ("context") weights of one block (modules.py:763-846; Attention *_c, modules.py:411-432).
+ * The last block (context_pre_only) has no to_out_c and no ff_c: w_out_c .. b_ff2_c are NULL there. */
+typedef struct {
+  const void* w_qkv_c; const float* b_qkv_c;     /* fp16 [3*inner, D] (to_q_c | to_k_c | to_v_c), fp32 [3*inner] */
+  const void* w_out_c; const float* b_out_c;     /* fp16 [D, inner] */
+  const void* w_ff1_c; const float* b_ff1_c;     /* fp16 [F, D] */
+  const void* w_ff2_c; const float* b_ff2_c;     /* fp16 [D, F] */
+  const float* q_norm_c; const float* k_norm_c;  /* arch.qk_norm: fp32 [dim_head] attn.c_q_norm / c_k_norm, else NULL */
+} f5_ctx_layer_weights;
+
 typedef struct {
   const void* time_w0; const float* time_b0;  /* fp16 [D, 256] */
   const void* time_w1; const float* time_b1;  /* fp16 [D, D] */
@@ -185,6 +208,14 @@ typedef struct {
   const void* out_w; const float* out_b;      /* fp16 [mel, D] proj_out */
   const void* long_skip_w;                    /* arch.long_skip: fp16 [D, 2D] long_skip_connection.weight
                                                  (backbones/dit.py:228, no bias), else NULL */
+  /* MMDiT (backbone 2) only, since f5_version() 107; read only then.
+   *   text_table  fp32 [V+1, D] text_embed.text_embed.weight;  proj_w  audio_embed.linear, K = 2*mel zero-padded to
+   *   proj_kpad (a multiple of 64);  conv_w / conv_b  audio_embed.conv_pos_embed;  layers[i]  the audio stream (to_q/k/v,
+   *   to_out.0, ff_x, q_norm / k_norm);  mod_w  every AdaLN linear stacked, per block [attn_norm_x: 6D | attn_norm_c:
+   *   6D, or 2D (scale, shift) in the last block], then norm_out 2D.
+   * Text padding must be trailing (as list_str_to_idx pads); the valid text length of each sample is the number of ids
+   * that are not -1, counted on the device. */
+  const f5_ctx_layer_weights* ctx_layers;     /* [depth] */
 } f5_weights;
 
 typedef struct f5_engine f5_engine;
@@ -213,13 +244,21 @@ typedef struct {
                                 218).  Euler makes `steps` backbone evaluations, midpoint 2 * steps (at t_k and at
                                 t_k + dt_k/2).  Any other value is rejected. */
 } f5_sample_args;
-/* nfe: backbone evaluations of the call — steps for euler, 2 * steps for midpoint */
+/* nfe: backbone evaluations of the call — steps for euler, 2 * steps for midpoint.  For MMDiT this is the workspace of
+ * a call with nt = N (an upper bound whenever nt < N, as CFM.sample gives for text from list_str_to_idx). */
 size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, float cfg_strength);
+/* The workspace of a call with text length nt; equals f5_sample_workspace_bytes for DiT and UNetT.  f5_sample rejects
+ * a workspace smaller than this for its nt.  Since f5_version() 107. */
+size_t f5_sample_workspace_bytes_nt(const f5_engine* e, int B, int N, int nt, int nfe, float cfg_strength);
 int f5_sample(f5_engine* e, const f5_sample_args* args, void* workspace, size_t ws_bytes, f5_stream_t stream);
 
 /* algorithmic FLOPs of one f5_sample call making nfe backbone evaluations (SURVEY.md §8d formula) — used by bench.py
  * for the roofline */
 double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength);
+/* f5_sample_flops at text length nt: for MMDiT it counts the text stream and the joint attention over N + nt keys;
+ * for DiT and UNetT it equals f5_sample_flops.  f5_sample_flops of an MMDiT engine is this at nt = N.  Since
+ * f5_version() 107. */
+double f5_sample_flops_nt(const f5_engine* e, int B, int N, int nt, int nfe, float cfg_strength);
 
 #ifdef __cplusplus
 }

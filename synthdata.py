@@ -20,7 +20,7 @@ import torch
 # ---------------------------------------------------------------------------
 @dataclass
 class ArchConfig:
-    backbone: str = "DiT"  # "DiT" | "UNetT"
+    backbone: str = "DiT"  # "DiT" | "UNetT" | "MMDiT" (MMDiT ignores text_dim, conv_layers and pe_attn_head)
     dim: int = 1024
     depth: int = 22
     heads: int = 16
@@ -78,6 +78,10 @@ def f5tts_v1_base_all_options() -> ArchConfig:  # F5TTS_v1_Base with qk_norm, lo
                       text_embedding_average_upsampling=True)
 
 
+def mmdit_v1_base_widths() -> ArchConfig:  # an MMDiT at F5TTS_v1_Base widths (no shipped config builds one)
+    return ArchConfig(backbone="MMDiT", text_dim=None, conv_layers=0, text_mask_padding=True, pe_attn_head=None)
+
+
 def f5tts_v1_base_dh128() -> ArchConfig:  # F5TTS_v1_Base with 8 heads of 128 (`heads: 8, dim_head: 128`)
     return ArchConfig(text_mask_padding=True, pe_attn_head=None, heads=8, dim_head=128)
 
@@ -90,6 +94,8 @@ def state_dict_spec(cfg: ArchConfig) -> list[tuple[str, tuple[int, ...], str]]:
 
     kind selects the synthetic distribution only.
     """
+    if cfg.backbone == "MMDiT":
+        return _mmdit_state_dict_spec(cfg)
     D, T, M = cfg.dim, cfg.tdim, cfg.mel_dim
     inner = cfg.heads * cfg.dim_head
     ff = int(D * cfg.ff_mult)
@@ -154,6 +160,51 @@ def state_dict_spec(cfg: ArchConfig) -> list[tuple[str, tuple[int, ...], str]]:
         lin(p + "proj_out", M, D)
     else:
         raise ValueError(cfg.backbone)
+    return spec
+
+
+def _mmdit_state_dict_spec(cfg: ArchConfig) -> list[tuple[str, tuple[int, ...], str]]:
+    """CFM(transformer=MMDiT) (backbones/mmdit.py:85-156; MMDiTBlock modules.py:763-804).  text_dim, conv_layers,
+    pe_attn_head and the DiT options do not exist there and are ignored."""
+    D, M = cfg.dim, cfg.mel_dim
+    inner, ff = cfg.heads * cfg.dim_head, int(D * cfg.ff_mult)
+    spec: list[tuple[str, tuple[int, ...], str]] = []
+
+    def lin(prefix, out_f, in_f, kind="linear"):
+        spec.extend([(prefix + ".weight", (out_f, in_f), kind), (prefix + ".bias", (out_f,), "bias")])
+
+    p = "transformer."
+    lin(p + "time_embed.time_mlp.0", D, 256)
+    lin(p + "time_embed.time_mlp.2", D, D)
+    spec.append((p + "text_embed.text_embed.weight", (cfg.text_num_embeds + 1, D), "embed"))
+    lin(p + "audio_embed.linear", D, 2 * M)
+    for i in (0, 2):
+        spec.append((f"{p}audio_embed.conv_pos_embed.conv1d.{i}.weight", (D, D // 16, 31), "conv"))
+        spec.append((f"{p}audio_embed.conv_pos_embed.conv1d.{i}.bias", (D,), "bias"))
+    spec.append((p + "rotary_embed.inv_freq", (cfg.dim_head // 2,), "inv_freq"))
+    for i in range(cfg.depth):
+        b, last = f"{p}transformer_blocks.{i}.", i == cfg.depth - 1  # last block: context_pre_only
+        lin(b + "attn_norm_c.linear", (2 if last else 6) * D, D, kind="adaln")
+        lin(b + "attn_norm_x.linear", 6 * D, D, kind="adaln")
+        for nm in ("to_q", "to_k", "to_v"):
+            lin(b + "attn." + nm, inner, D)
+        if cfg.qk_norm is not None:
+            spec.append((b + "attn.q_norm.weight", (cfg.dim_head,), "ln_w"))
+            spec.append((b + "attn.k_norm.weight", (cfg.dim_head,), "ln_w"))
+        for nm in ("to_q_c", "to_k_c", "to_v_c"):
+            lin(b + "attn." + nm, inner, D)
+        if cfg.qk_norm is not None:
+            spec.append((b + "attn.c_q_norm.weight", (cfg.dim_head,), "ln_w"))
+            spec.append((b + "attn.c_k_norm.weight", (cfg.dim_head,), "ln_w"))
+        lin(b + "attn.to_out.0", D, inner)
+        if not last:
+            lin(b + "attn.to_out_c", D, inner)
+            lin(b + "ff_c.ff.0.0", ff, D)
+            lin(b + "ff_c.ff.2", D, ff)
+        lin(b + "ff_x.ff.0.0", ff, D)
+        lin(b + "ff_x.ff.2", D, ff)
+    lin(p + "norm_out.linear", 2 * D, D, kind="adaln")
+    lin(p + "proj_out", M, D)
     return spec
 
 
