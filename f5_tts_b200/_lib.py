@@ -44,7 +44,7 @@ class VocosWeights(C.Structure):
 class Arch(C.Structure):
     _fields_ = [(n, c_int) for n in ("backbone", "dim", "depth", "heads", "dim_head", "ff_inner", "mel_dim", "text_dim",
                                      "text_num_embeds", "conv_layers", "text_mask_padding", "pe_attn_head",
-                                     "attn_mask_enabled", "qk_norm", "long_skip", "text_avg_upsample")]
+                                     "attn_mask_enabled", "qk_norm", "long_skip", "text_avg_upsample", "skip_type")]
 
 
 class LayerWeights(C.Structure):
@@ -85,6 +85,7 @@ class SampleArgs(C.Structure):
 
 ODE_METHODS = {"euler": 0, "midpoint": 1}
 BACKBONES = {"DiT": 0, "UNetT": 1, "MMDiT": 2}  # Arch.backbone  # SampleArgs.method; backbone evaluations per grid interval: 1 and 2
+SKIP_TYPES = {"concat": 0, "add": 1, "none": 2}  # Arch.skip_type: UNetT skip_connect_type
 
 
 _lock = threading.Lock()
@@ -170,5 +171,5 @@ KERNEL_HOOK_SYMBOLS = [
     "f5k_last_error", "f5k_row_norm", "f5k_dwconv7_ln", "f5k_text_gather", "f5k_mask_rows", "f5k_mask_rows_len",
     "f5k_grn_rows", "f5k_grn", "f5k_pack_input", "f5k_cfg_euler", "f5k_small_linear", "f5k_time_features",
     "f5k_silu_to_half", "f5k_rope_table", "f5k_prepend_time_token", "f5k_concat_half", "f5k_vocos_im2col",
-    "f5k_ln_affine_f32", "f5k_istft",
+    "f5k_ln_affine_f32", "f5k_istft", "f5k_row_norm_add_skip",
 ]

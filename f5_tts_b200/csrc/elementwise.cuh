@@ -12,16 +12,19 @@ namespace f5 {
 //   MODE 0: LayerNorm(eps, no affine) * (1 + scale[c]) + shift[c]     (modules.py:312-326, 333-347, 753)
 //   MODE 1: LayerNorm(eps) * w[c] + b[c]                               (ConvNeXt / Vocos norms)
 //   MODE 2: x / max(||x||, 1e-12) * sqrt(D) * g[c]                     (x_transformers RMSNorm, unett.py:154)
+//   MODE 3: x += skip (fp32, written back to x), then MODE 2 of the sum (UNetT skip_connect_type="add": the
+//           `x = x + skip` that opens each later-half layer fused into its attn_norm, unett.py:296-297)
 // scale/shift live in the per-step modulation table: ptr + (*step_ptr) * step_stride.
 // ---------------------------------------------------------------------------------------------------------
 
 template <int MODE>
 __global__ void __launch_bounds__(256) row_norm_kernel(const NormParams p) {
+  constexpr bool kAffine = MODE == 0 || MODE == 1;  // LayerNorm with a second parameter row (shift / bias)
   pdl_launch_dependents();
   const int row = blockIdx.x * int(blockDim.x >> 5) + (threadIdx.x >> 5);  // one warp per row
   const int lane = lane_id();
   const int nv = p.D >> 7;  // float4 per lane (D multiple of 128, <= 1024)
-  float4 v[8], ga[8], gb[8];
+  float4 v[8], ga[8], gb[8];  // gb: shift / bias row (MODE 0, 1) or the skip row (MODE 3)
   float s = 0.f;
   // Scale / shift of this step: inside the engine they were written long before the producer of x (modulation table,
   // step counter of the previous NFE step), so they are fetched BEFORE the programmatic-launch dependency wait — the
@@ -29,12 +32,12 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const NormParams p) {
   auto load_params = [&]() {
     const long long so = p.step_ptr ? (long long)(*p.step_ptr) * p.step_stride : 0;
     const float4* A = reinterpret_cast<const float4*>(p.a + so);
-    const float4* B = (MODE == 2) ? nullptr : reinterpret_cast<const float4*>(p.b + so);
+    const float4* B = kAffine ? reinterpret_cast<const float4*>(p.b + so) : nullptr;
 #pragma unroll
     for (int i = 0; i < 8; ++i)
       if (i < nv) {
         ga[i] = __ldg(A + i * 32 + lane);
-        if (MODE != 2) gb[i] = __ldg(B + i * 32 + lane);
+        if (kAffine) gb[i] = __ldg(B + i * 32 + lane);
       }
   };
   if (p.params_static && row < p.rows) load_params();
@@ -45,12 +48,32 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const NormParams p) {
 #pragma unroll
   for (int i = 0; i < 8; ++i)
     if (i < nv) v[i] = xr[i * 32 + lane];
+  if (MODE == 3) {
+    // the skip row was saved layers ago, but it is read after the dependency wait like x: nothing before the wait may
+    // rely on work older than the producer having finished
+    const float4* sr = reinterpret_cast<const float4*>(p.skip + (long long)row * p.D);
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (i < nv) gb[i] = sr[i * 32 + lane];
+  }
   if (!p.params_static) load_params();
+  if (MODE == 3) {
+    float4* xw = const_cast<float4*>(xr);  // x is read-write in this mode only
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (i < nv) {
+        v[i].x += gb[i].x;
+        v[i].y += gb[i].y;
+        v[i].z += gb[i].z;
+        v[i].w += gb[i].w;
+        xw[i * 32 + lane] = v[i];
+      }
+  }
 #pragma unroll
   for (int i = 0; i < 8; ++i)
     if (i < nv) s += v[i].x + v[i].y + v[i].z + v[i].w;
   float mean = 0.f, rstd;
-  if (MODE != 2) {
+  if (kAffine) {
     mean = warp_sum(s) / float(p.D);
     float q = 0.f;
 #pragma unroll

@@ -132,6 +132,7 @@ struct f5_engine {
 };
 
 static constexpr int kMMDiT = 2;
+static constexpr int kSkipConcat = 0, kSkipAdd = 1, kSkipNone = 2;  // f5_arch.skip_type (UNetT skip_connect_type)
 
 // MMDiT: first row of block i's modulation vectors in the AdaLN table ([x: 6D | c: 6D] per block, the last block's c
 // part 2D, then norm_out 2D); DiT: [6D] per block, then norm_out
@@ -176,9 +177,11 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.c1 = bp.take<__half>((size_t)L.M * D);
   L.skips.clear();
   if (A.backbone == 1) {
+    // concat and add keep the depth/2 saved rows; only concat has the [x | skip] operand of its combiner GEMM
     L.x = bp.take<float>((size_t)L.M1 * D);
-    for (int i = 0; i < A.depth / 2; ++i) L.skips.push_back(bp.take<float>((size_t)L.M1 * D));
-    L.cat = bp.take<__half>((size_t)L.M1 * 2 * D);
+    if (A.skip_type != kSkipNone)
+      for (int i = 0; i < A.depth / 2; ++i) L.skips.push_back(bp.take<float>((size_t)L.M1 * D));
+    L.cat = A.skip_type == kSkipConcat ? bp.take<__half>((size_t)L.M1 * 2 * D) : nullptr;
   } else {
     L.x = L.h0;
     L.cat = nullptr;
@@ -278,6 +281,30 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
     set_error("engine_create: long_skip needs long_skip_w");
     return -1;
   }
+  if (arch->skip_type < kSkipConcat || arch->skip_type > kSkipNone || (arch->skip_type && arch->backbone != 1)) {
+    set_error("engine_create: skip_type must be 0 (concat), 1 (add) or 2 (none), and non-zero only for UNetT "
+              "(backbone %d, skip_type %d)", arch->backbone, arch->skip_type);
+    return -1;
+  }
+  if (arch->backbone == 1 && arch->skip_type != kSkipConcat) {
+    // every first-half layer pushes x and every later-half layer pops one (unett.py:286-294): an odd depth pops more
+    // than it pushed
+    if (arch->depth % 2) {
+      set_error("engine_create: UNetT skip_type add / none needs an even depth (got %d)", arch->depth);
+      return -1;
+    }
+    for (int i = 0; i < arch->depth; ++i)
+      if (weights->layers[i].w_skip != nullptr) {
+        set_error("engine_create: UNetT skip_type add / none has no skip projection, but layer %d has w_skip", i);
+        return -1;
+      }
+  }
+  if (arch->backbone == 1 && arch->skip_type == kSkipConcat)
+    for (int i = arch->depth / 2; i < arch->depth; ++i)
+      if (weights->layers[i].w_skip == nullptr) {
+        set_error("engine_create: UNetT skip_type concat needs w_skip in every later-half layer (layer %d)", i);
+        return -1;
+      }
   if (arch->qk_norm)
     for (int i = 0; i < arch->depth; ++i)
       if (weights->layers[i].q_norm_w == nullptr || weights->layers[i].k_norm_w == nullptr) {
@@ -355,7 +382,9 @@ double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_stre
     if (A.long_skip) per += 2.0 * n * D * (2.0 * D);  // long_skip_connection: Linear(2D -> D)
   } else {
     const double n1 = N + 1.0, n = N;
-    per = Ld * (8.0 * n1 * D * I + 4.0 * n1 * D * F + 4.0 * n1 * n1 * I) + (Ld / 2.0) * 4.0 * n1 * D * D +
+    // concat: the combiner Linear(2D -> D) of every later-half layer; add and none have no GEMM there
+    const double combiner = A.skip_type == kSkipConcat ? (Ld / 2.0) * 4.0 * n1 * D * D : 0.0;
+    per = Ld * (8.0 * n1 * D * I + 4.0 * n1 * D * F + 4.0 * n1 * n1 * I) + combiner +
           2.0 * n * (2 * mel + Td) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n1 * D * mel;
   }
   double total = nfe * Be * per;
@@ -527,8 +556,10 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
   // In the default "faithful" mode padded keys ARE attended (SURVEY.md §0.5) and every row must be computed.
   const int key_mask = (masked && (A.attn_mask_enabled || strict)) ? 1 : 0;
   // MMDiT's conv position embedding reads padded audio rows (no mask, mmdit.py:67-78), and those rows evolve with the
-  // ODE like any other: outside exact_varlen they must be computed in full
-  const int skip = mmdit ? (strict ? 1 : 0) : key_mask;
+  // ODE like any other: outside exact_varlen they must be computed in full.  UNetT's conv is unmasked too
+  // (unett.py:90-102); add and none compute every row the same way, concat keeps the tile skipping it always had.
+  const bool unmasked_conv = mmdit || (A.backbone == 1 && A.skip_type != kSkipConcat);
+  const int skip = unmasked_conv ? (strict ? 1 : 0) : key_mask;
   auto varlen = [&](f5_gemm_args& a) {
     if (!skip) return;
     a.row_len = L.row_len;
@@ -638,8 +669,9 @@ static constexpr bool diag_skip(const char*) { return false; }
 #endif
 
 int norm_mod(const f5_engine* e, const Layout& L, const float* x, long long rows, int mode, const float* a,
-             const float* b, bool step_indexed, cudaStream_t s, __half* out = nullptr) {
+             const float* b, bool step_indexed, cudaStream_t s, __half* out = nullptr, const float* skip = nullptr) {
   NormParams p{};
+  p.skip = skip;
   p.x = x;
   p.out = out ? out : L.a;
   p.rows = (int)rows;
@@ -712,14 +744,19 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
       const float* m = L.mod + (size_t)i * 6 * D;
       RC(norm_mod(e, L, L.x, L.M1, 0, m + D, m, true, s));  // scale_msa, shift_msa
     } else {
-      if (i < half) {
-        RC(check_cuda(cudaMemcpyAsync(L.skips[i], L.x, sizeof(float) * L.M1 * D, cudaMemcpyDeviceToDevice, s),
-                      "skip copy"));
+      if (A.skip_type == kSkipAdd && i >= half) {
+        // x += skip and attn_norm in one pass over the rows (row norm mode 3)
+        RC(norm_mod(e, L, L.x, L.M1, 3, lw.g_attn, nullptr, false, s, nullptr, L.skips[A.depth - 1 - i]));
       } else {
-        RC(run_concat_half(L.x, L.skips[A.depth - 1 - i], L.cat, L.M1, D, s));
-        RC(gemm_run(P.skip[i], s));
+        if (A.skip_type != kSkipNone && i < half) {
+          RC(check_cuda(cudaMemcpyAsync(L.skips[i], L.x, sizeof(float) * L.M1 * D, cudaMemcpyDeviceToDevice, s),
+                        "skip copy"));
+        } else if (A.skip_type == kSkipConcat) {
+          RC(run_concat_half(L.x, L.skips[A.depth - 1 - i], L.cat, L.M1, D, s));
+          RC(gemm_run(P.skip[i], s));
+        }
+        RC(norm_mod(e, L, L.x, L.M1, 2, lw.g_attn, nullptr, false, s));
       }
-      RC(norm_mod(e, L, L.x, L.M1, 2, lw.g_attn, nullptr, false, s));
     }
     if (!diag_skip("qkv")) RC(gemm_run(P.qkv[i], s));
     if (!diag_skip("attn")) RC(attn_run(P.attn[0], s));

@@ -16,6 +16,7 @@ struct NormParams {
   const int* step_ptr;
   long long step_stride;
   int params_static;  // a / b / *step_ptr were not written by the kernel preceding this launch: fetch them before the PDL wait
+  const float* skip;  // MODE 3: [rows, D] added to x; the sum is written back to x (x is read-write in that mode)
 };
 
 struct DwConvLnParams {

@@ -30,6 +30,20 @@ int f5k_row_norm(int mode, const float* x, void* out, int rows, int D, float eps
   return run_row_norm(mode, p, st(s));
 }
 
+// row norm mode 3: x += skip in place, out = RMSNorm(x) * g
+int f5k_row_norm_add_skip(float* x, const float* skip, void* out, int rows, int D, const float* g, void* s) {
+  NormParams p{};
+  p.x = x;
+  p.skip = skip;
+  p.out = reinterpret_cast<__half*>(out);
+  p.rows = rows;
+  p.D = D;
+  p.eps = 1e-6f;
+  p.a = g;
+  p.params_static = 1;
+  return run_row_norm(3, p, st(s));
+}
+
 int f5k_dwconv7_ln(const float* x, void* out, int B, int N, int C, const float* w, const float* wb, const float* ln_w,
                    const float* ln_b, float eps, void* s) {
   DwConvLnParams p{};

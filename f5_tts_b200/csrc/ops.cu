@@ -58,7 +58,11 @@ int run_row_norm(int mode, const NormParams& p, cudaStream_t s) {
   if (mode == 0) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<0>, p);
   else if (mode == 1) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<1>, p);
   else if (mode == 2) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<2>, p);
-  else {
+  else if (mode == 3 && p.skip != nullptr) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<3>, p);
+  else if (mode == 3) {
+    set_error("row_norm: mode 3 needs the skip rows");
+    return -1;
+  } else {
     set_error("row_norm: bad mode %d", mode);
     return -1;
   }

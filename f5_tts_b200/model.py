@@ -134,7 +134,7 @@ def _mmdit_spec(*, dim, depth, heads, dim_head, ff_mult, mel_dim, text_num_embed
 
 
 def _backbone_spec(kind: str, *, dim, depth, heads, dim_head, ff_mult, mel_dim, text_num_embeds, text_dim,
-                   conv_layers, qk_norm=None, long_skip_connection=False):
+                   conv_layers, qk_norm=None, long_skip_connection=False, skip_connect_type="concat"):
     """(key, shape, init) for every tensor of the backbone; identical names to dit.py / unett.py / mmdit.py modules."""
     if kind == "MMDiT":
         return _mmdit_spec(dim=dim, depth=depth, heads=heads, dim_head=dim_head, ff_mult=ff_mult, mel_dim=mel_dim,
@@ -180,7 +180,7 @@ def _backbone_spec(kind: str, *, dim, depth, heads, dim_head, ff_mult, mel_dim, 
     else:
         for i in range(depth):
             b = f"layers.{i}."
-            if i >= depth // 2:
+            if i >= depth // 2 and skip_connect_type == "concat":  # slot 0 is None otherwise (unett.py:146, 171)
                 lin(b + "0", D, 2 * D, bias=False)
             out.append((b + "1.g", (D,), "one"))
             for nm in ("to_q", "to_k", "to_v"):
@@ -214,6 +214,7 @@ def _nfe(steps: int, method: str) -> int:
 
 
 DIM_HEADS = (64, 128)  # attention head widths the kernels are built for
+SKIP_CONNECT_TYPES = ("concat", "add", "none")  # UNetT skip_connect_type (unett.py:127)
 
 
 class _Backbone(nn.Module):
@@ -234,9 +235,12 @@ class _Backbone(nn.Module):
             raise TypeError("text_embedding_average_upsampling and long_skip_connection are DiT arguments")
         if avg_up:  # the reference's TextEmbedding asserts it (dit.py:41-43)
             assert text_mask_padding, "text_embedding_average_upsampling requires text_mask_padding to be True"
-        skip = unsupported.pop("skip_connect_type", "concat")
-        if skip != "concat":
-            raise NotImplementedError("UNetT skip_connect_type other than 'concat' is not built")
+        skip = unsupported.pop("skip_connect_type", "concat" if self.KIND == "UNetT" else None)
+        if skip is not None and self.KIND != "UNetT":
+            raise TypeError("skip_connect_type is a UNetT argument")
+        if self.KIND == "UNetT":
+            if skip not in SKIP_CONNECT_TYPES:  # the reference runs any other string like "none" (unett.py:290-297)
+                raise ValueError(f"skip_connect_type must be one of {SKIP_CONNECT_TYPES}, got {skip!r}")
         if qk_norm not in (None, "rms_norm"):
             raise ValueError(f"Unimplemented qk_norm: {qk_norm}")  # modules.py:408-409
         if unsupported:
@@ -256,10 +260,12 @@ class _Backbone(nn.Module):
         self.attn_backend = attn_backend  # accepted for config compatibility; the H100 kernel is always used
         # long_skip: the flag (`long_skip_connection` is the Linear's module name, as in dit.py:228)
         self.qk_norm, self.long_skip, self.text_embedding_average_upsampling = qk_norm, long_skip, avg_up
+        self.skip_connect_type = skip  # UNetT: "concat" | "add" | "none"; None for DiT and MMDiT
         for key, shape, how in _backbone_spec(self.KIND, dim=dim, depth=depth, heads=heads, dim_head=dim_head,
                                               ff_mult=ff_mult, mel_dim=mel_dim, text_num_embeds=text_num_embeds,
                                               text_dim=text_dim, conv_layers=conv_layers, qk_norm=qk_norm,
-                                              long_skip_connection=long_skip):
+                                              long_skip_connection=long_skip,
+                                              skip_connect_type=skip or "concat"):
             _attach(self, key, _init_tensor(shape, how))
         inv_freq = 1.0 / (10000 ** (torch.arange(0, dim_head, 2).float() / dim_head))
         _attach(self, "rotary_embed.inv_freq", inv_freq, buffer=True)
@@ -390,7 +396,8 @@ class DiT(_Backbone):
 
 
 class UNetT(_Backbone):
-    """backbones/unett.py:108-128"""
+    """backbones/unett.py:108-128.  skip_connect_type "concat" (default), "add" or "none"; "add" and "none" need an even
+    depth, which the engine checks when it is first created (at the first sample)."""
 
     KIND = "UNetT"
 

@@ -181,6 +181,7 @@ def engine_from_packed(m, T: dict[str, torch.Tensor]) -> dict:
     A.qk_norm = 1 if m.qk_norm is not None else 0
     A.long_skip = 1 if m.long_skip else 0
     A.text_avg_upsample = 1 if m.text_embedding_average_upsampling else 0
+    A.skip_type = _lib.SKIP_TYPES[m.skip_connect_type] if m.KIND == "UNetT" else 0
     handle = C.c_void_p()
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().f5_engine_create(C.byref(A), C.byref(W), C.byref(handle)), "f5_engine_create")
@@ -206,6 +207,8 @@ def cache_key(ckpt_path: str, m) -> str:
     options = (m.qk_norm, m.long_skip, m.text_embedding_average_upsampling)
     if any(options):  # appended only when an option is on: packed caches of other models keep their keys
         arch += options
+    if m.KIND == "UNetT" and m.skip_connect_type != "concat":  # likewise: concat models keep their keys
+        arch += (f"skip_connect_type={m.skip_connect_type}",)
     raw = f"{os.path.abspath(ckpt_path)}|{st.st_size}|{st.st_mtime_ns}|{arch}|fmt{PACK_FORMAT}"
     return hashlib.sha256(raw.encode()).hexdigest()[:24]
 

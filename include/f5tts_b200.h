@@ -166,6 +166,11 @@ typedef struct {
                             cat(x after the last block, x after the input embedding) before norm_out */
   int text_avg_upsample; /* DiT text_embedding_average_upsampling (backbones/dit.py:41-84, 131-137): each sample's
                             valid text tokens spread evenly over its audio length; needs text_mask_padding */
+  /* Since f5_version() 108.  UNetT skip_connect_type (backbones/unett.py:127, 290-297): how each later-half layer
+   * combines x with the x its mirror first-half layer saved.  0 = "concat": x = w_skip . cat(x, skip), w_skip needed in
+   * every later-half layer; 1 = "add": x = x + skip; 2 = "none": the saved x is not used.  1 and 2 take no w_skip and
+   * need an even depth.  Non-zero only for UNetT; a zeroed struct gets 0, the engine before this field. */
+  int skip_type;
 } f5_arch;
 
 typedef struct {
@@ -173,7 +178,7 @@ typedef struct {
   const void* w_out; const float* b_out;   /* fp16 [D, inner] */
   const void* w_ff1; const float* b_ff1;   /* fp16 [F, D] */
   const void* w_ff2; const float* b_ff2;   /* fp16 [D, F] */
-  const void* w_skip;                      /* UNetT later half: fp16 [D, 2D], else NULL */
+  const void* w_skip;                      /* UNetT later half with skip_type 0: fp16 [D, 2D], else NULL */
   const float* g_attn; const float* g_ff;  /* UNetT RMSNorm gains */
   const float* q_norm_w; const float* k_norm_w; /* arch.qk_norm: fp32 [dim_head] attn.q_norm / k_norm weight
                                                    (modules.py:406-407), else NULL */

@@ -37,6 +37,7 @@ class ArchConfig:
     qk_norm: Optional[str] = None  # None | "rms_norm"
     long_skip_connection: bool = False
     text_embedding_average_upsampling: bool = False
+    skip_connect_type: str = "concat"  # UNetT: "concat" | "add" | "none" (backbones/unett.py:127)
 
     @property
     def tdim(self) -> int:
@@ -144,7 +145,7 @@ def state_dict_spec(cfg: ArchConfig) -> list[tuple[str, tuple[int, ...], str]]:
     elif cfg.backbone == "UNetT":
         for i in range(cfg.depth):
             b = f"{p}layers.{i}."
-            if i >= cfg.depth // 2:
+            if i >= cfg.depth // 2 and cfg.skip_connect_type == "concat":  # skip_proj (unett.py:146, 171)
                 lin(b + "0", D, 2 * D, bias=False)
             spec.append((b + "1.g", (D,), "ln_w"))
             for nm in ("to_q", "to_k", "to_v"):
