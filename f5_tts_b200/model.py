@@ -25,7 +25,7 @@ import torch.nn.functional as F
 from torch import nn
 from torch.nn.utils.rnn import pad_sequence
 
-from . import _lib
+from . import _lib, batching
 
 # ----------------------------------------------------------------------------------------------------------------
 # small host helpers (model/utils.py)
@@ -476,6 +476,9 @@ class MelSpec(nn.Module):
 # ----------------------------------------------------------------------------------------------------------------
 # sampler
 # ----------------------------------------------------------------------------------------------------------------
+_rng_lock = threading.Lock()  # torch's global generators, seeded per call by sample(seed=...)
+
+
 class CFM(nn.Module):
     """model/cfm.py:34-81 constructor; only `sample` (inference) is on this path — `forward` (training loss) is not."""
 
@@ -497,6 +500,22 @@ class CFM(nn.Module):
         self.odeint_kwargs = odeint_kwargs
         self.vocab_char_map = vocab_char_map
         self.use_cuda_graph = True
+        self.batcher = None  # a batching.SampleBatcher while enable_batching() is on
+
+    def enable_batching(self, max_batch: int = batching.DEFAULT_MAX_BATCH,
+                        max_frames: int = batching.DEFAULT_MAX_FRAMES) -> batching.BatchStats:
+        """Merge concurrent `sample()` calls on this model into shared engine calls (f5_tts_b200/batching.py).
+
+        Calls of one sample, or of several with `exact_varlen=True`, that share the time grid (steps, sway, EPSS,
+        duplicate_test), `cfg_strength`, the ODE method and `use_cuda_graph` run as one exact_varlen engine call of at
+        most `max_batch` samples and `max_frames` samples x padded frames; each caller gets bit for bit what its own call
+        returns.  A call that finds no other in flight runs at once.  Returns the batcher's counters."""
+        self.batcher = batching.SampleBatcher(self.transformer, max_batch=max_batch, max_frames=max_frames)
+        return self.batcher.stats
+
+    def disable_batching(self):
+        """Every later `sample()` call runs its own engine call again (calls already waiting are still served)."""
+        self.batcher = None
 
     @property
     def device(self):
@@ -557,10 +576,11 @@ class CFM(nn.Module):
 
         if y0 is None:  # same RNG calls as cfm.py:196-201
             rows = []
-            for dur in duration:
-                if exists(seed):
-                    torch.manual_seed(seed)
-                rows.append(torch.randn(int(dur), self.num_channels, device=self.device, dtype=step_cond.dtype))
+            with _rng_lock:  # concurrent calls: a seed and the draws it seeds are not interleaved with another call's
+                for dur in duration:
+                    if exists(seed):
+                        torch.manual_seed(seed)
+                    rows.append(torch.randn(int(dur), self.num_channels, device=self.device, dtype=step_cond.dtype))
             y0 = pad_sequence(rows, padding_value=0, batch_first=True)
         t_start = 0
         if duplicate_test:
@@ -577,9 +597,10 @@ class CFM(nn.Module):
 
         y = y0.float().contiguous().clone()
         trajectory = torch.empty((steps + 1, batch, n_frames, self.num_channels), device=device, dtype=torch.float32)
-        self.transformer.run(y, step_cond.float().contiguous(), text.to(torch.int64).contiguous(), t.tolist(), dur32,
-                             cfg_strength, trajectory=trajectory, use_graph=self.use_cuda_graph,
-                             exact_varlen=exact_varlen, method=self.odeint_kwargs.get("method", "euler"))
+        runner = self.transformer if self.batcher is None else self.batcher  # the batcher may merge this call
+        runner.run(y, step_cond.float().contiguous(), text.to(torch.int64).contiguous(), t.tolist(), dur32,
+                   cfg_strength, trajectory=trajectory, use_graph=self.use_cuda_graph,
+                   exact_varlen=exact_varlen, method=self.odeint_kwargs.get("method", "euler"))
         self.transformer.clear_cache()
 
         out = torch.where(cond_mask, cond, trajectory[-1].to(dtype))

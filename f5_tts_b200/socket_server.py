@@ -13,7 +13,9 @@ of a connection is cut again at half and then a quarter of that size so that the
 What differs from the reference, by necessity of this image: model architectures come from ``api.MODEL_ARCH`` (no
 hydra / omegaconf), the reference wave is read with the stdlib reader of ``infer._load_wav`` (no torchaudio codec),
 checkpoints / vocoder are local paths (no network).  Sampling runs through ``infer.infer_batch_process(...,
-streaming=True)``, i.e. the same kernels as every other entry point.
+streaming=True)``, i.e. the same kernels as every other entry point.  Each client's chunks are B = 1 sampler calls made
+from that client's thread; ``--batch_clients`` merges the calls of concurrent clients into shared engine calls
+(``CFM.enable_batching``); the wire protocol is unchanged and each call computes what it would compute alone.
 """
 from __future__ import annotations
 
@@ -197,10 +199,14 @@ def main():
     ap.add_argument("--ref_text", required=True)
     ap.add_argument("--device", default=None)
     ap.add_argument("--dtype", default=torch.float32)
+    ap.add_argument("--batch_clients", action="store_true",
+                    help="merge the sampler calls of concurrent clients into shared engine calls (CFM.enable_batching)")
     a = ap.parse_args()
     logging.basicConfig(level=logging.INFO)
     proc = TTSStreamingProcessor(a.model, a.ckpt_file, a.vocab_file, a.ref_audio, a.ref_text, device=a.device,
                                  dtype=a.dtype, vocoder_local_path=a.vocoder_local_path, output_file="output.wav")
+    if a.batch_clients:
+        proc.model.enable_batching()
     start_server(a.host, a.port, proc)
 
 
