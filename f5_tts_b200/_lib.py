@@ -138,9 +138,13 @@ def lib():
         L.f5_sample_workspace_bytes_nt.restype = c_size_t
         L.f5_sample_flops_nt.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_float]
         L.f5_sample_flops_nt.restype = C.c_double
+        L.f5_sample_cfg_split.argtypes = [c_void_p, C.POINTER(SampleArgs), c_void_p, c_size_t, c_void_p,
+                                          c_void_p, C.POINTER(SampleArgs), c_void_p, c_size_t, c_void_p]
+        L.f5_sample_cfg_split_workspace_bytes.argtypes = [c_void_p, c_int, c_int, c_int, c_int]
+        L.f5_sample_cfg_split_workspace_bytes.restype = c_size_t
         for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_attention_joint", "f5_row_norm", "f5_mel_spectrogram",
                      "f5_vocos_decode",
-                     "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample"):
+                     "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample", "f5_sample_cfg_split"):
             getattr(L, name).restype = c_int
         _lib = L
     return _lib
@@ -161,7 +165,7 @@ EXPORTED_SYMBOLS = [
     "f5_row_norm", "f5_mel_spectrogram",
     "f5_vocos_workspace_bytes", "f5_vocos_decode", "f5_vocos_decode_varlen", "f5_engine_create", "f5_engine_destroy",
     "f5_sample_workspace_bytes", "f5_sample", "f5_sample_flops", "f5_attention_joint", "f5_sample_workspace_bytes_nt",
-    "f5_sample_flops_nt",
+    "f5_sample_flops_nt", "f5_sample_cfg_split", "f5_sample_cfg_split_workspace_bytes",
 ]
 
 # Test-only library: the same objects plus one extern "C" wrapper per kernel launcher (csrc/kernel_hooks.cu), used by

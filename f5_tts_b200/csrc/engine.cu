@@ -48,6 +48,10 @@ struct Bump {
 struct Layout {
   // sizes
   int B, Be, N, seq, evals, packed;  // evals: backbone evaluations per call (steps, or 2 * steps for midpoint)
+  // CFG split (f5_sample_cfg_split): -1 = both halves stacked on the batch axis (f5_sample); 0 / 1 = this workspace
+  // computes only the conditional / unconditional half: Be = B rows of work, while xin, v and the MMDiT text embedding
+  // keep both halves (Bx = 2B samples) so that the unchanged update kernel runs over the full v
+  int half, Bx;
   long long M, M1;
   // common
   int* step_ptr;    // [0]: evaluation counter
@@ -68,22 +72,26 @@ struct Layout {
   __half *ta, *tg;
   float *sumsq, *nx;
   // step buffers
-  __half* xin;
+  __half* xin;      // this half's rows of xin_all (= xin_all unless split)
+  __half* xin_all;  // [Bx*N, kin]
   float* h0;
   __half *h0h, *c1;
   float* x;                  // UNetT residual [M1, D]; DiT: alias of h0
   std::vector<float*> skips;
   __half* cat;
   __half *a, *qkv, *ao, *g;
-  float* v;
+  float* v;      // this half's rows of v_all (= v_all unless split)
+  float* v_all;  // [Bx*seq, mel]: cond rows, then uncond rows
   float* x_embed;  // DiT long_skip_connection: x after the input embedding [M1, D] (cat(...) goes to `cat`), else null
   float* txu;      // text_embedding_average_upsampling: upsampled text [2B, N, Td], else null
   // MMDiT text stream (null for DiT / UNetT): nt tokens per sample
   int nt;
   float *c, *c0;               // [Be*nt, D] residual; the text embedding it restarts from at every evaluation
+  float* c0_all;               // [Bx*nt, D] text embedding of both CFG variants (c0 points at this half's rows)
   __half *ac, *qkv_c, *ao_c, *g_c;  // normalised copy, QKV, attention output, FF hidden
   float *c_rope_cos, *c_rope_sin;   // [nt, dim_head / 2]
-  int* c_len;                  // [Be] valid text tokens per sample
+  int* c_len;                  // [Be] valid text tokens per sample (this half's entries of c_len_all [Bx])
+  int* c_len_all;
   size_t bytes;
 };
 
@@ -111,9 +119,11 @@ struct GraphKey {
   int B, N, evals, packed, masked;  // masked: 0 = no lengths, 1 = lengths (reference batched semantics), 2 = exact_varlen
   int nt;  // MMDiT: the text length sets the text-stream layout and plans.  0 for DiT / UNetT, whose graphs do not
            // depend on it (keying them on it would re-capture whenever text lengths differ)
+  int half;  // Layout::half: -1 for f5_sample's graph (the whole evaluation), 0 / 1 for one CFG half of a split call
+             // (the evaluation up to proj_out: the exchange and the update run outside the graph)
   bool operator==(const GraphKey& o) const {
     return ws == o.ws && B == o.B && N == o.N && evals == o.evals && packed == o.packed && masked == o.masked &&
-           nt == o.nt;
+           nt == o.nt && half == o.half;
   }
 };
 struct GraphEntry {
@@ -138,14 +148,17 @@ static constexpr int kSkipConcat = 0, kSkipAdd = 1, kSkipNone = 2;  // f5_arch.s
 // part 2D, then norm_out 2D); DiT: [6D] per block, then norm_out
 static size_t mod_block(const f5_arch& A, int i) { return (size_t)i * (A.backbone == kMMDiT ? 12 : 6) * A.dim; }
 
-static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int nt, int evals, float cfg) {
+static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int nt, int evals, float cfg,
+                        int half = -1) {
   const f5_arch& A = e->arch;
   Bump bp(ws);
   L.B = B;
   L.N = N;
   L.evals = evals;
-  L.packed = cfg < 1e-5f ? 0 : 1;
-  L.Be = L.packed ? 2 * B : B;
+  L.half = half;
+  L.packed = (cfg < 1e-5f && half < 0) ? 0 : 1;
+  L.Be = (L.packed && half < 0) ? 2 * B : B;
+  L.Bx = L.packed ? 2 * B : B;
   L.seq = A.backbone == 1 ? N + 1 : N;
   L.M = (long long)L.Be * N;
   L.M1 = (long long)L.Be * L.seq;
@@ -171,7 +184,8 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.tg = bp.take<__half>((size_t)2 * B * N * 2 * Td);
   L.sumsq = bp.take<float>((size_t)2 * B * ((N + kGrnRows - 1) / kGrnRows) * 2 * Td);
   L.nx = bp.take<float>((size_t)2 * B * 2 * Td);
-  L.xin = bp.take<__half>((size_t)L.M * e->kin);
+  L.xin_all = bp.take<__half>((size_t)L.Bx * N * e->kin);
+  L.xin = L.xin_all + (half > 0 ? (size_t)B * N * e->kin : 0);
   L.h0 = bp.take<float>((size_t)L.M * D);
   L.h0h = bp.take<__half>((size_t)L.M * D);
   L.c1 = bp.take<__half>((size_t)L.M * D);
@@ -190,7 +204,8 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.qkv = bp.take<__half>((size_t)L.M1 * 3 * e->inner);
   L.ao = bp.take<__half>((size_t)L.M1 * e->inner);
   L.g = bp.take<__half>((size_t)L.M1 * F);
-  L.v = bp.take<float>((size_t)L.M1 * A.mel_dim);
+  L.v_all = bp.take<float>((size_t)L.Bx * L.seq * A.mel_dim);
+  L.v = L.v_all + (half > 0 ? (size_t)B * L.seq * A.mel_dim : 0);
   // buffers of the architecture options last: with the options off the layout is the one above
   L.x_embed = nullptr;
   if (A.long_skip) {
@@ -199,21 +214,23 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   }
   L.txu = A.text_avg_upsample ? bp.take<float>((size_t)2 * B * N * Td) : nullptr;
   L.nt = nt;
-  L.c = L.c0 = nullptr;
+  L.c = L.c0 = L.c0_all = nullptr;
   L.ac = L.qkv_c = L.ao_c = L.g_c = nullptr;
   L.c_rope_cos = L.c_rope_sin = nullptr;
-  L.c_len = nullptr;
+  L.c_len = L.c_len_all = nullptr;
   if (A.backbone == kMMDiT) {
     const size_t Mc = (size_t)L.Be * nt;
     L.c = bp.take<float>(Mc * D);
-    L.c0 = bp.take<float>(Mc * D);
+    L.c0_all = bp.take<float>((size_t)L.Bx * nt * D);
+    L.c0 = L.c0_all + (half > 0 ? (size_t)B * nt * D : 0);
     L.ac = bp.take<__half>(Mc * D);
     L.qkv_c = bp.take<__half>(Mc * 3 * e->inner);
     L.ao_c = bp.take<__half>(Mc * e->inner);
     L.g_c = bp.take<__half>(Mc * F);
     L.c_rope_cos = bp.take<float>((size_t)nt * (A.dim_head / 2));
     L.c_rope_sin = bp.take<float>((size_t)nt * (A.dim_head / 2));
-    L.c_len = bp.take<int>(L.Be);
+    L.c_len_all = bp.take<int>(L.Bx);
+    L.c_len = L.c_len_all + (half > 0 ? B : 0);
   }
   L.bytes = bp.off + 512;
 }
@@ -714,7 +731,8 @@ int run_mmdit_block(f5_engine* e, const Layout& L, const StepPlans& P, int i, cu
   return gemm_run(P.ff2[i], s);
 }
 
-int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const StepPlans& P, cudaStream_t s) {
+// One backbone evaluation up to and including proj_out: v (this layout's half of it when split) holds the flow
+int run_body(f5_engine* e, const Layout& L, const StepPlans& P, cudaStream_t s) {
   const f5_arch& A = e->arch;
   const int D = A.dim;
   const bool dit = A.backbone == 0;
@@ -780,11 +798,16 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
   } else {
     RC(norm_mod(e, L, L.x, L.M1, 2, e->w.g_out, nullptr, false, s));
   }
-  RC(gemm_run(P.out_proj, s));
+  return gemm_run(P.out_proj, s);
+}
+
+// The fused CFG + ODE stage update over the full v (both halves), rewriting the x columns of every row of xin
+int run_update(const f5_engine* e, const Layout& L, cudaStream_t s) {
+  const f5_arch& A = e->arch;
   EulerParams ep{};
   ep.io = L.io;
-  ep.v = L.v;
-  ep.xin = L.xin;
+  ep.v = L.v_all;
+  ep.xin = L.xin_all;
   ep.stage = L.stage;
   ep.step_ptr = L.step_ptr;
   ep.BN = L.B * L.N;
@@ -796,6 +819,11 @@ int run_step(f5_engine* e, const Layout& L, const f5_sample_args* sa, const Step
   ep.tok_off = A.backbone == 1 ? 1 : 0;
   ep.B = L.B;
   return run_cfg_euler(ep, s);
+}
+
+int run_step(f5_engine* e, const Layout& L, const StepPlans& P, cudaStream_t s) {
+  RC(run_body(e, L, P, s));
+  return run_update(e, L, s);
 }
 
 int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaStream_t s) {
@@ -870,8 +898,8 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     RC(gemm_run(pl, s));
   }
   if (mmdit) {  // text embedding of both CFG variants and the text rope table; no text columns in the input projection
-    RC(run_mmdit_text_embed(sa->text, B, L.Be, L.nt, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding, L.c0,
-                            L.c_len, s));
+    RC(run_mmdit_text_embed(sa->text, B, L.Bx, L.nt, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding,
+                            L.c0_all, L.c_len_all, s));
     RC(run_rope_table(L.c_rope_cos, L.c_rope_sin, L.nt, A.dim_head / 2, s));
   }
   // text embedding, both CFG variants (dit.py:86-139 / unett.py:55-84)
@@ -923,7 +951,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   if (A.text_avg_upsample)  // audio lengths: duration (the reference's seq_len = mask.sum), else N
     RC(run_text_avg_upsample(L.tx, L.txu, L.filler, masked ? L.valid_len : nullptr, B, N, sa->nt, Td, s));
   PackParams pp{};
-  pp.xin = L.xin;
+  pp.xin = L.xin_all;
   pp.B = B;
   pp.N = N;
   pp.mel = A.mel_dim;
@@ -944,10 +972,72 @@ int copy_v_out(const f5_engine* e, const Layout& L, const f5_sample_args* sa, cu
   if (!sa->v_out) return 0;
   const int mel = e->arch.mel_dim;
   const int off = e->arch.backbone == 1 ? 1 : 0;
-  for (int b = 0; b < L.Be; ++b)
-    RC(check_cuda(cudaMemcpyAsync(sa->v_out + (size_t)b * L.N * mel, L.v + ((size_t)b * L.seq + off) * mel,
+  for (int b = 0; b < L.Bx; ++b)
+    RC(check_cuda(cudaMemcpyAsync(sa->v_out + (size_t)b * L.N * mel, L.v_all + ((size_t)b * L.seq + off) * mel,
                                   sizeof(float) * L.N * mel, cudaMemcpyDeviceToDevice, s),
                   "v_out copy"));
+  return 0;
+}
+
+// The step graph of this (workspace, shapes, half): from the engine's cache, or captured now on the current device.
+int step_graph(f5_engine* e, const Layout& L, const f5_sample_args* sa, const void* ws,
+               std::shared_ptr<GraphHolder>* out) {
+  const GraphKey key{ws, sa->B, sa->N, L.evals, L.packed, sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1),
+                     e->arch.backbone == kMMDiT ? sa->nt : 0, L.half};
+  std::shared_ptr<GraphHolder> g;
+  {
+    std::lock_guard<std::mutex> lk(e->mu);
+    for (auto& en : e->graphs)
+      if (en.key == key) g = en.g;
+  }
+  if (!g) {
+    // Capture outside the engine mutex (thread-local capture mode: concurrent sample() calls capture independently)
+    // on a private stream — the caller's stream may be the legacy default stream, which cannot capture.
+    StepPlans P;
+    RC(build_step_plans(e, L, sa, P));
+    cudaStream_t cs;
+    RC(check_cuda(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking), "capture stream"));
+    if (int brc = check_cuda(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal), "begin capture")) {
+      cudaStreamDestroy(cs);
+      return brc;
+    }
+    const unsigned long long before = f5_launch_count();
+    const int rc = L.half < 0 ? run_step(e, L, P, cs) : run_body(e, L, P, cs);
+    cudaGraph_t graph = nullptr;
+    const cudaError_t ce = cudaStreamEndCapture(cs, &graph);
+    cudaStreamDestroy(cs);
+    count_launch(-(int)(f5_launch_count() - before));  // captured, not launched
+    if (rc || ce != cudaSuccess) {
+      if (graph) cudaGraphDestroy(graph);
+      return rc ? rc : check_cuda(ce, "end capture");
+    }
+    g = std::make_shared<GraphHolder>();
+    size_t nn = 0;
+    cudaGraphGetNodes(graph, nullptr, &nn);
+    g->nodes = (int)nn;
+    const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (ie != cudaSuccess) {
+      g->exec = nullptr;
+      return check_cuda(ie, "graph instantiate");
+    }
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (e->graphs.size() >= 16) e->graphs.erase(e->graphs.begin());  // holder is freed when its last user is done
+    e->graphs.push_back(GraphEntry{key, g});
+  }
+  *out = std::move(g);
+  return 0;
+}
+
+int check_problem(const char* fn, const f5_sample_args* sa) {
+  if (sa->B <= 0 || sa->N <= 0 || sa->steps <= 0 || sa->nt <= 0) {
+    set_error("%s: empty problem (B=%d N=%d steps=%d nt=%d)", fn, sa->B, sa->N, sa->steps, sa->nt);
+    return -1;
+  }
+  if (sa->method != 0 && sa->method != 1) {
+    set_error("%s: method must be 0 (euler) or 1 (midpoint), got %d", fn, sa->method);
+    return -1;
+  }
   return 0;
 }
 
@@ -959,14 +1049,7 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
     set_error("f5_sample: null argument");
     return -1;
   }
-  if (sa->B <= 0 || sa->N <= 0 || sa->steps <= 0 || sa->nt <= 0) {
-    set_error("f5_sample: empty problem (B=%d N=%d steps=%d nt=%d)", sa->B, sa->N, sa->steps, sa->nt);
-    return -1;
-  }
-  if (sa->method != 0 && sa->method != 1) {
-    set_error("f5_sample: method must be 0 (euler) or 1 (midpoint), got %d", sa->method);
-    return -1;
-  }
+  RC(check_problem("f5_sample", sa));
   const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
   Layout L;
   plan_layout(e, L, workspace, sa->B, sa->N, sa->nt, evals, sa->cfg_strength);
@@ -976,55 +1059,228 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
   }
   RC(run_prologue(e, L, sa, s));
   if (sa->use_graph) {
-    const GraphKey key{workspace, sa->B, sa->N, evals, L.packed,
-                       sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1), e->arch.backbone == kMMDiT ? sa->nt : 0};
     std::shared_ptr<GraphHolder> g;
-    {
-      std::lock_guard<std::mutex> lk(e->mu);
-      for (auto& en : e->graphs)
-        if (en.key == key) g = en.g;
-    }
-    if (!g) {
-      // Capture outside the engine mutex (thread-local capture mode: concurrent sample() calls capture independently)
-      // on a private stream — the caller's stream may be the legacy default stream, which cannot capture.
-      StepPlans P;
-      RC(build_step_plans(e, L, sa, P));
-      cudaStream_t cs;
-      RC(check_cuda(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking), "capture stream"));
-      if (int brc = check_cuda(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal), "begin capture")) {
-        cudaStreamDestroy(cs);
-        return brc;
-      }
-      const unsigned long long before = f5_launch_count();
-      const int rc = run_step(e, L, sa, P, cs);
-      cudaGraph_t graph = nullptr;
-      const cudaError_t ce = cudaStreamEndCapture(cs, &graph);
-      cudaStreamDestroy(cs);
-      count_launch(-(int)(f5_launch_count() - before));  // captured, not launched
-      if (rc || ce != cudaSuccess) {
-        if (graph) cudaGraphDestroy(graph);
-        return rc ? rc : check_cuda(ce, "end capture");
-      }
-      g = std::make_shared<GraphHolder>();
-      size_t nn = 0;
-      cudaGraphGetNodes(graph, nullptr, &nn);
-      g->nodes = (int)nn;
-      const cudaError_t ie = cudaGraphInstantiate(&g->exec, graph, 0);
-      cudaGraphDestroy(graph);
-      if (ie != cudaSuccess) {
-        g->exec = nullptr;
-        return check_cuda(ie, "graph instantiate");
-      }
-      std::lock_guard<std::mutex> lk(e->mu);
-      if (e->graphs.size() >= 16) e->graphs.erase(e->graphs.begin());  // holder is freed when its last user is done
-      e->graphs.push_back(GraphEntry{key, g});
-    }
+    RC(step_graph(e, L, sa, workspace, &g));
     for (int k = 0; k < evals; ++k) RC(check_cuda(cudaGraphLaunch(g->exec, s), "graph launch"));
     count_launch(g->nodes * evals);
     return copy_v_out(e, L, sa, s);
   }
   StepPlans P;
   RC(build_step_plans(e, L, sa, P));
-  for (int k = 0; k < evals; ++k) RC(run_step(e, L, sa, P, s));
+  for (int k = 0; k < evals; ++k) RC(run_step(e, L, P, s));
   return copy_v_out(e, L, sa, s);
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// CFG split (f5_sample_cfg_split): the conditional half of the packed batch on one workspace, the unconditional half on
+// another, usually on another device.  The halves share nothing inside a backbone evaluation; they meet only in the
+// update g = pred + (pred - null) * cfg.  So per evaluation k each side runs its half up to proj_out (run_body), pulls
+// the other side's half of v into its own full v, and runs the unchanged update kernel over the full v: both sides
+// then hold the same y and the same x columns of xin, and the next evaluation starts from identical inputs.
+//
+// Ordering, with s_d the stream of side d and o the other side.  Per evaluation k, host order:
+//   pass 1, each d:  [k > 0] s_d waits pulled_o       (o's pull of d's v from evaluation k-1 is done)
+//                    run_body on s_d                   (writes d's half of v_d)
+//                    record ready_d on s_d
+//   pass 2, each d:  s_d waits ready_o                 (o's half of v_o is complete)
+//                    copy o's half of v_o -> v_d       (on s_d)
+//                    record pulled_d on s_d
+//                    run_update on s_d                 (reads both halves of v_d)
+// Each buffer is written on one stream only; the cross-stream hazards are the copy's source, v_o's half on o: read
+// after o wrote it (ready_o) and before o overwrites it at k+1 (o waits pulled_d before its next run_body).  The copy's
+// destination is d's own v, read only by d's update, later on s_d.  At the end each stream waits for the other's last
+// pull, so neither workspace is reused while the other side still reads it.  Every wait is enqueued after the record it
+// refers to (pass 1 of k waits on pass 2 of k-1, pass 2 on pass 1 of k), so a wait never refers to work that was not
+// issued: if a side fails partway and the host stops, a wait on an event whose record was never issued refers to the
+// previous record or none, and does not block.  No kernel waits on a flag written by the other side.
+namespace {
+
+struct SplitSide {
+  f5_engine* e;
+  const f5_sample_args* sa;
+  void* ws;
+  size_t bytes;
+  cudaStream_t s;
+  int dev = -1;
+  Layout L;
+  StepPlans P;
+  std::shared_ptr<GraphHolder> g;
+  cudaEvent_t ready = nullptr, pulled = nullptr;
+};
+
+int pointer_device(const void* p, const char* what, int* dev) {
+  cudaPointerAttributes at{};
+  RC(check_cuda(cudaPointerGetAttributes(&at, p), what));
+  if (at.type != cudaMemoryTypeDevice) {
+    set_error("f5_sample_cfg_split: %s is not device memory", what);
+    return -1;
+  }
+  *dev = at.device;
+  return 0;
+}
+
+// Direct copies between the two devices where the hardware allows it (a per-process context setting, made once per
+// ordered pair); otherwise cudaMemcpyPeerAsync stages through the host.
+int enable_peer_access(int dev, int peer) {
+  static std::mutex mu;
+  static std::vector<std::pair<int, int>> done;
+  std::lock_guard<std::mutex> lk(mu);
+  for (auto& p : done)
+    if (p.first == dev && p.second == peer) return 0;
+  int can = 0;
+  RC(check_cuda(cudaDeviceCanAccessPeer(&can, dev, peer), "cudaDeviceCanAccessPeer"));
+  if (can) {
+    RC(check_cuda(cudaSetDevice(dev), "cudaSetDevice"));
+    const cudaError_t err = cudaDeviceEnablePeerAccess(peer, 0);
+    if (err == cudaErrorPeerAccessAlreadyEnabled)
+      cudaGetLastError();  // enabled before (by this library or by the caller): not an error
+    else
+      RC(check_cuda(err, "cudaDeviceEnablePeerAccess"));
+  }
+  done.emplace_back(dev, peer);
+  return 0;
+}
+
+int split_check(const SplitSide* sd) {
+  const f5_sample_args *a = sd[0].sa, *b = sd[1].sa;
+  if (a->B != b->B || a->N != b->N || a->nt != b->nt || a->steps != b->steps || a->method != b->method ||
+      a->use_graph != b->use_graph || a->exact_varlen != b->exact_varlen || a->cfg_strength != b->cfg_strength ||
+      (a->duration == nullptr) != (b->duration == nullptr)) {
+    set_error("f5_sample_cfg_split: the two argument blocks must describe the same problem (B, N, nt, steps, method, "
+              "use_graph, exact_varlen, cfg_strength, duration given or not)");
+    return -1;
+  }
+  for (int k = 0; k <= a->steps; ++k)
+    if (a->t[k] != b->t[k]) {
+      set_error("f5_sample_cfg_split: the two time grids differ at %d", k);
+      return -1;
+    }
+  if (a->cfg_strength < 1e-5f) {
+    set_error("f5_sample_cfg_split: cfg_strength %g has no unconditional half to split off", a->cfg_strength);
+    return -1;
+  }
+  if (b->trajectory || b->v_out) {
+    set_error("f5_sample_cfg_split: only the first side writes trajectory and v_out");
+    return -1;
+  }
+  if (a->y == b->y || sd[0].s == sd[1].s) {
+    set_error("f5_sample_cfg_split: each side needs its own y and its own stream");
+    return -1;
+  }
+  if (std::memcmp(&sd[0].e->arch, &sd[1].e->arch, sizeof(f5_arch)) != 0) {
+    set_error("f5_sample_cfg_split: the two engines have different architectures");
+    return -1;
+  }
+  const uint8_t *w0 = static_cast<const uint8_t*>(sd[0].ws), *w1 = static_cast<const uint8_t*>(sd[1].ws);
+  if (w0 < w1 + sd[1].bytes && w1 < w0 + sd[0].bytes) {
+    set_error("f5_sample_cfg_split: the two workspaces overlap");
+    return -1;
+  }
+  return 0;
+}
+
+int split_loop(SplitSide* sd, int evals) {
+  const size_t half_floats = (size_t)sd[0].L.B * sd[0].L.seq * sd[0].e->arch.mel_dim;
+  for (int k = 0; k < evals; ++k) {
+    for (int d = 0; d < 2; ++d) {
+      SplitSide &me = sd[d], &o = sd[1 - d];
+      RC(check_cuda(cudaSetDevice(me.dev), "cudaSetDevice"));
+      if (k > 0) RC(check_cuda(cudaStreamWaitEvent(me.s, o.pulled, 0), "wait pulled"));
+      if (me.g) {
+        RC(check_cuda(cudaGraphLaunch(me.g->exec, me.s), "graph launch"));
+        count_launch(me.g->nodes);
+      } else {
+        RC(run_body(me.e, me.L, me.P, me.s));
+      }
+      RC(check_cuda(cudaEventRecord(me.ready, me.s), "record ready"));
+    }
+    for (int d = 0; d < 2; ++d) {
+      SplitSide &me = sd[d], &o = sd[1 - d];
+      RC(check_cuda(cudaSetDevice(me.dev), "cudaSetDevice"));
+      RC(check_cuda(cudaStreamWaitEvent(me.s, o.ready, 0), "wait ready"));
+      RC(check_cuda(cudaMemcpyPeerAsync(me.L.v_all + (o.L.v - o.L.v_all), me.dev, o.L.v, o.dev,
+                                        sizeof(float) * half_floats, me.s),
+                    "v exchange"));
+      RC(check_cuda(cudaEventRecord(me.pulled, me.s), "record pulled"));
+      RC(run_update(me.e, me.L, me.s));
+    }
+  }
+  return 0;
+}
+
+int split_run(SplitSide* sd) {
+  const f5_sample_args* sa = sd[0].sa;
+  const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
+  for (int d = 0; d < 2; ++d) {
+    SplitSide& me = sd[d];
+    plan_layout(me.e, me.L, me.ws, sa->B, sa->N, sa->nt, evals, sa->cfg_strength, d);
+    if (me.bytes < me.L.bytes) {
+      set_error("f5_sample_cfg_split: workspace %d too small (%zu < %zu)", d, me.bytes, me.L.bytes);
+      return -1;
+    }
+  }
+  if (sd[0].dev != sd[1].dev) {
+    RC(enable_peer_access(sd[0].dev, sd[1].dev));
+    RC(enable_peer_access(sd[1].dev, sd[0].dev));
+  }
+  for (int d = 0; d < 2; ++d) {
+    SplitSide& me = sd[d];
+    RC(check_cuda(cudaSetDevice(me.dev), "cudaSetDevice"));
+    RC(check_cuda(cudaEventCreateWithFlags(&me.ready, cudaEventDisableTiming), "event create"));
+    RC(check_cuda(cudaEventCreateWithFlags(&me.pulled, cudaEventDisableTiming), "event create"));
+    RC(run_prologue(me.e, me.L, me.sa, me.s));
+    if (sa->use_graph)
+      RC(step_graph(me.e, me.L, me.sa, me.ws, &me.g));
+    else
+      RC(build_step_plans(me.e, me.L, me.sa, me.P));
+  }
+  return split_loop(sd, evals);
+}
+
+}  // namespace
+
+extern "C" size_t f5_sample_cfg_split_workspace_bytes(const f5_engine* e, int B, int N, int nt, int nfe) {
+  Layout L;
+  plan_layout(e, L, nullptr, B, N, nt, nfe, 1.0f, 0);  // both halves have the same layout
+  return L.bytes;
+}
+
+extern "C" int f5_sample_cfg_split(f5_engine* e0, const f5_sample_args* a0, void* ws0, size_t ws0_bytes,
+                                   f5_stream_t stream0, f5_engine* e1, const f5_sample_args* a1, void* ws1,
+                                   size_t ws1_bytes, f5_stream_t stream1) {
+  if (!e0 || !a0 || !ws0 || !e1 || !a1 || !ws1) {
+    set_error("f5_sample_cfg_split: null argument");
+    return -1;
+  }
+  RC(check_problem("f5_sample_cfg_split", a0));
+  SplitSide sd[2];
+  sd[0].e = e0, sd[0].sa = a0, sd[0].ws = ws0, sd[0].bytes = ws0_bytes, sd[0].s = reinterpret_cast<cudaStream_t>(stream0);
+  sd[1].e = e1, sd[1].sa = a1, sd[1].ws = ws1, sd[1].bytes = ws1_bytes, sd[1].s = reinterpret_cast<cudaStream_t>(stream1);
+  RC(split_check(sd));
+  RC(pointer_device(ws0, "workspace 0", &sd[0].dev));
+  RC(pointer_device(ws1, "workspace 1", &sd[1].dev));
+  int caller_dev = 0;
+  RC(check_cuda(cudaGetDevice(&caller_dev), "cudaGetDevice"));
+  int rc = split_run(sd);
+  // Also after a failure: each stream waits for the other side's last pull (a no-op for an event never recorded), so
+  // neither workspace is handed back while the other side may still read it.  Then the events go (destroying an event
+  // with work pending is allowed: its resources are released once that work completes).
+  for (int d = 0; d < 2; ++d) {
+    SplitSide &me = sd[d], &o = sd[1 - d];
+    if (!me.ready || !o.pulled) continue;
+    const cudaError_t err = cudaSetDevice(me.dev) != cudaSuccess ? cudaErrorInvalidDevice
+                                                                  : cudaStreamWaitEvent(me.s, o.pulled, 0);
+    if (!rc) rc = check_cuda(err, "final wait");
+  }
+  if (!rc) {
+    cudaSetDevice(sd[0].dev);
+    rc = copy_v_out(e0, sd[0].L, a0, sd[0].s);
+  }
+  for (int d = 0; d < 2; ++d) {
+    cudaSetDevice(sd[d].dev);
+    if (sd[d].ready) cudaEventDestroy(sd[d].ready);
+    if (sd[d].pulled) cudaEventDestroy(sd[d].pulled);
+  }
+  cudaSetDevice(caller_dev);
+  return rc;
 }

@@ -384,7 +384,7 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 
 extern "C" {
 
-int f5_version(void) { return 108; }
+int f5_version(void) { return 109; }
 const char* f5_last_error(void) { return f5::g_err; }
 unsigned long long f5_launch_count(void) { return f5::g_launches.load(); }
 

@@ -25,7 +25,7 @@ import torch.nn.functional as F
 from torch import nn
 from torch.nn.utils.rnn import pad_sequence
 
-from . import _lib, batching
+from . import _lib, batching, cfg_parallel
 
 # ----------------------------------------------------------------------------------------------------------------
 # small host helpers (model/utils.py)
@@ -273,6 +273,7 @@ class _Backbone(nn.Module):
         self._engine_state = None
         self._ws_lock = threading.Lock()
         self._ws_free: dict = {}  # (device, stream) -> [uint8 tensors] not in use by a sample() call
+        self.cfg_peer = None  # a cfg_parallel.CfgPeer while CFM.enable_cfg_parallel() is on
 
     # -- engine management ------------------------------------------------------------------------------------
     def _fingerprint(self):
@@ -333,7 +334,18 @@ class _Backbone(nn.Module):
     def run(self, y, step_cond, text, t_grid, duration, cfg_strength, trajectory=None, v_out=None, use_graph=True,
             exact_varlen=False, method="euler"):
         """One engine call = len(t_grid)-1 steps of the fixed-grid ODE `method` ("euler": one backbone evaluation per
-        step, "midpoint": two).  All tensors on the CUDA device, fp32 / int64 / int32."""
+        step, "midpoint": two).  All tensors on the CUDA device, fp32 / int64 / int32.  With a CFG peer set
+        (CFM.enable_cfg_parallel) a call with guidance runs its unconditional half there; one without (cfg_strength
+        < 1e-5) or one that asks for the raw backbone output (v_out) runs here alone."""
+        peer = self.cfg_peer
+        if peer is not None and v_out is None and float(cfg_strength) >= 1e-5:
+            return peer.run(self, y, step_cond, text, t_grid, duration, cfg_strength, trajectory, use_graph,
+                            exact_varlen, method)
+        return self._run_local(y, step_cond, text, t_grid, duration, cfg_strength, trajectory, v_out, use_graph,
+                               exact_varlen, method)
+
+    def _run_local(self, y, step_cond, text, t_grid, duration, cfg_strength, trajectory=None, v_out=None,
+                   use_graph=True, exact_varlen=False, method="euler"):
         st = self.engine()
         L = _lib.lib()
         B, N, mel = y.shape
@@ -382,8 +394,8 @@ class _Backbone(nn.Module):
         duration = None if mask is None else mask.sum(dim=1).to(torch.int32).contiguous()
         packed = cfg_infer or drop_text
         v = torch.empty((2 * B if packed else B, N, mel), device=dev, dtype=torch.float32)
-        self.run(y, sc, text.to(torch.int64).contiguous(), [t0, t0 + 1.0], duration, 1.0 if packed else 0.0, None, v,
-                 use_graph=False)
+        self._run_local(y, sc, text.to(torch.int64).contiguous(), [t0, t0 + 1.0], duration, 1.0 if packed else 0.0,
+                        None, v, use_graph=False)
         if cfg_infer:
             return v.to(x.dtype)
         return (v[B:] if drop_text else v).to(x.dtype)
@@ -516,6 +528,28 @@ class CFM(nn.Module):
     def disable_batching(self):
         """Every later `sample()` call runs its own engine call again (calls already waiting are still served)."""
         self.batcher = None
+
+    def enable_cfg_parallel(self, device) -> cfg_parallel.CfgPeer:
+        """Run the unconditional half of every guided `sample()` call on `device` (f5_tts_b200/cfg_parallel.py).
+
+        The conditional half stays on the model's device; after each backbone evaluation the two devices exchange their
+        halves of the flow and both apply the same update, so every call returns bit for bit what it returns without
+        this.  `device` holds a replica of the backbone's packed weights, copied again when the weights change; it may be
+        the model's own device (two workspaces on one GPU).  Calls with cfg_strength < 1e-5 and the backbone's
+        `forward` stay on the model's device.  Merged runs of `enable_batching` split too.  ValueError for a CPU or
+        unknown device.  Enabling it again for the same device keeps the peer (its weight copy, stream, workspaces and
+        captured graphs).  Returns the peer."""
+        dev = cfg_parallel.peer_device(device)
+        peer = self.transformer.cfg_peer
+        if peer is None or peer.device != dev:
+            peer = cfg_parallel.CfgPeer(dev)
+            self.transformer.cfg_peer = peer
+        return peer
+
+    def disable_cfg_parallel(self) -> None:
+        """Later `sample()` calls run on the model's device alone again; the peer's weight copy and workspaces go once
+        no call uses them."""
+        self.transformer.cfg_peer = None
 
     @property
     def device(self):

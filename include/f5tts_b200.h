@@ -257,6 +257,22 @@ size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, floa
 size_t f5_sample_workspace_bytes_nt(const f5_engine* e, int B, int N, int nt, int nfe, float cfg_strength);
 int f5_sample(f5_engine* e, const f5_sample_args* args, void* workspace, size_t ws_bytes, f5_stream_t stream);
 
+/* One f5_sample call with classifier-free guidance split over two engines: side 0 computes the conditional half of every
+ * backbone evaluation, side 1 the unconditional half, and after each evaluation each side copies the other's half of
+ * the flow (B * N * mel fp32 values) into its own workspace and runs the same fused CFG + ODE update.  Both sides then
+ * hold the same y; the final y, trajectory and v_out are bit for bit those of f5_sample(e0, a0, ...).
+ *   e1 may be e0 (two workspaces on one device) or an engine over the same weights on another device, each workspace
+ *   on its engine's device (the device is read from the workspace pointer).  a0 and a1 describe the same problem (B, N,
+ *   nt, steps, t, cfg_strength >= 1e-5, method, use_graph, exact_varlen, durations given or not); a1's text, step_cond,
+ *   y and duration are copies on side 1's device, its y a buffer of its own, its trajectory and v_out NULL.
+ *   stream0 and stream1 must differ; the call is ordered after earlier work on each stream and completes on both: each
+ *   stream waits for the other side's last read of its workspace.  Peer access between the two devices is enabled
+ *   once per process where the hardware allows it.  Since f5_version() 109. */
+int f5_sample_cfg_split(f5_engine* e0, const f5_sample_args* a0, void* ws0, size_t ws0_bytes, f5_stream_t stream0,
+                        f5_engine* e1, const f5_sample_args* a1, void* ws1, size_t ws1_bytes, f5_stream_t stream1);
+/* workspace of either side of f5_sample_cfg_split (nfe as for f5_sample_workspace_bytes).  Since f5_version() 109. */
+size_t f5_sample_cfg_split_workspace_bytes(const f5_engine* e, int B, int N, int nt, int nfe);
+
 /* algorithmic FLOPs of one f5_sample call making nfe backbone evaluations (SURVEY.md §8d formula) — used by bench.py
  * for the roofline */
 double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength);
