@@ -88,6 +88,25 @@ BACKBONES = {"DiT": 0, "UNetT": 1, "MMDiT": 2}  # Arch.backbone  # SampleArgs.me
 SKIP_TYPES = {"concat": 0, "add": 1, "none": 2}  # Arch.skip_type: UNetT skip_connect_type
 
 
+def sample_args(y, step_cond, text, duration, tg, steps, cfg_strength, trajectory, use_graph, exact_varlen, method,
+                v_out=None) -> SampleArgs:
+    """The f5_sample argument block of one call over these tensors.  `tg` is the ctypes float array of the time grid;
+    the block points into it, so it must outlive the call."""
+    a = SampleArgs()
+    B, N, _ = y.shape
+    a.B, a.N, a.nt, a.steps = B, N, text.shape[1], steps
+    a.text, a.step_cond, a.y = text.data_ptr(), step_cond.data_ptr(), y.data_ptr()
+    a.duration = duration.data_ptr() if duration is not None else None
+    a.t = tg
+    a.cfg_strength = float(cfg_strength)
+    a.trajectory = trajectory.data_ptr() if trajectory is not None else None
+    a.use_graph = 1 if use_graph else 0
+    a.v_out = v_out.data_ptr() if v_out is not None else None
+    a.exact_varlen = 1 if (exact_varlen and duration is not None) else 0
+    a.method = ODE_METHODS[method]
+    return a
+
+
 _lock = threading.Lock()
 _lib = None
 

@@ -56,22 +56,6 @@ def destroy(state: dict) -> None:
     _lib.lib().f5_engine_destroy(state["handle"])
 
 
-def _args(y, step_cond, text, duration, tg, steps, cfg_strength, trajectory, use_graph, exact_varlen, method):
-    a = _lib.SampleArgs()
-    B, N, _ = y.shape
-    a.B, a.N, a.nt, a.steps = B, N, text.shape[1], steps
-    a.text, a.step_cond, a.y = text.data_ptr(), step_cond.data_ptr(), y.data_ptr()
-    a.duration = duration.data_ptr() if duration is not None else None
-    a.t = tg
-    a.cfg_strength = float(cfg_strength)
-    a.trajectory = trajectory.data_ptr() if trajectory is not None else None
-    a.use_graph = 1 if use_graph else 0
-    a.v_out = None
-    a.exact_varlen = 1 if (exact_varlen and duration is not None) else 0
-    a.method = _lib.ODE_METHODS[method]
-    return a
-
-
 class CfgPeer:
     """The peer side of split calls for one backbone: the device, the replica engine, a stream, a workspace pool.
 
@@ -165,8 +149,9 @@ class CfgPeer:
             sc1, text1 = step_cond.to(self.device), text.to(self.device)
             dur1 = duration.to(self.device) if duration is not None else None
         tg = (C.c_float * (steps + 1))(*[float(v) for v in t_grid])
-        a0 = _args(y, step_cond, text, duration, tg, steps, cfg_strength, trajectory, use_graph, exact_varlen, method)
-        a1 = _args(y1, sc1, text1, dur1, tg, steps, cfg_strength, None, use_graph, exact_varlen, method)
+        a0 = _lib.sample_args(y, step_cond, text, duration, tg, steps, cfg_strength, trajectory, use_graph,
+                              exact_varlen, method)
+        a1 = _lib.sample_args(y1, sc1, text1, dur1, tg, steps, cfg_strength, None, use_graph, exact_varlen, method)
         ws0 = backbone._ws_acquire(need, dev0, caller.cuda_stream)
         ws1 = self._ws_acquire(need)
         try:

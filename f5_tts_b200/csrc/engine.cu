@@ -45,20 +45,31 @@ struct Bump {
   }
 };
 
+// One residual stream of the backbone: the audio rows, or MMDiT's text rows.  Every transformer block runs the same
+// norm -> QKV -> attention -> out-projection -> norm -> FF1 -> FF2 sequence over it.
+struct TokenStream {
+  float* res;                // residual [rows, D]
+  __half *a, *qkv, *ao, *g;  // normalised copy, QKV, attention output, FF hidden
+  long long rows;            // Be * seq
+  int seq;                   // tokens per sample
+  float *rope_cos, *rope_sin;  // [seq, dim_head / 2]
+  const int* out_len;   // [Be] valid rows of the out-projection (padded rows are zeroed), or null
+  const int* skip_len;  // [Be] valid rows when every GEMM skips tiles of padding only, or null
+};
+
 struct Layout {
   // sizes
-  int B, Be, N, seq, evals, packed;  // evals: backbone evaluations per call (steps, or 2 * steps for midpoint)
+  int B, Be, N, evals, packed;  // evals: backbone evaluations per call (steps, or 2 * steps for midpoint)
   // CFG split (f5_sample_cfg_split): -1 = both halves stacked on the batch axis (f5_sample); 0 / 1 = this workspace
   // computes only the conditional / unconditional half: Be = B rows of work, while xin, v and the MMDiT text embedding
   // keep both halves (Bx = 2B samples) so that the unchanged update kernel runs over the full v
   int half, Bx;
-  long long M, M1;
+  long long M;  // Be * N mel frames (the audio stream's rows without the UNetT time token)
   // common
   int* step_ptr;    // [0]: evaluation counter
   SampleIo* io;     // caller tensors + cfg scale of THIS call, read by the step kernels through the workspace
   OdeStage* stage;  // [evals]
   float* t_dev;     // [evals] evaluation times
-  float *rope_cos, *rope_sin;
   int* row_len;     // [Be] or unused
   int* kv_len;      // [Be] or unused
   int* frame_len;   // [Be] valid mel frames per sample (row_len without the UNetT time token)
@@ -76,21 +87,20 @@ struct Layout {
   __half* xin_all;  // [Bx*N, kin]
   float* h0;
   __half *h0h, *c1;
-  float* x;                  // UNetT residual [M1, D]; DiT: alias of h0
+  // audio stream: seq = N (+1 for the UNetT time token); residual is the UNetT residual, DiT / MMDiT: alias of h0.
+  // Its row lengths depend on the call's arguments and are set when the plans are built.
+  TokenStream x;
   std::vector<float*> skips;
   __half* cat;
-  __half *a, *qkv, *ao, *g;
   float* v;      // this half's rows of v_all (= v_all unless split)
   float* v_all;  // [Bx*seq, mel]: cond rows, then uncond rows
   float* x_embed;  // DiT long_skip_connection: x after the input embedding [M1, D] (cat(...) goes to `cat`), else null
   float* txu;      // text_embedding_average_upsampling: upsampled text [2B, N, Td], else null
-  // MMDiT text stream (null for DiT / UNetT): nt tokens per sample
-  int nt;
-  float *c, *c0;               // [Be*nt, D] residual; the text embedding it restarts from at every evaluation
-  float* c0_all;               // [Bx*nt, D] text embedding of both CFG variants (c0 points at this half's rows)
-  __half *ac, *qkv_c, *ao_c, *g_c;  // normalised copy, QKV, attention output, FF hidden
-  float *c_rope_cos, *c_rope_sin;   // [nt, dim_head / 2]
-  int* c_len;                  // [Be] valid text tokens per sample (this half's entries of c_len_all [Bx])
+  // MMDiT text stream (all null for DiT / UNetT): nt tokens per sample; out_len = c_len, no tile skipping
+  TokenStream c;
+  float* c0;      // [Be*nt, D] the text embedding the residual restarts from at every evaluation
+  float* c0_all;  // [Bx*nt, D] text embedding of both CFG variants (c0 points at this half's rows)
+  int* c_len;     // [Be] valid text tokens per sample (this half's entries of c_len_all [Bx])
   int* c_len_all;
   size_t bytes;
 };
@@ -135,18 +145,25 @@ struct f5_engine {
   f5_arch arch;
   f5_weights w;
   std::vector<f5_layer_weights> layers;
-  std::vector<f5_ctx_layer_weights> ctx;  // MMDiT text stream
+  std::vector<f5_layer_weights> ctx;  // MMDiT text stream (the f5_ctx_layer_weights in the same slots)
   int inner, modW, kin;
   std::mutex mu;
   std::vector<GraphEntry> graphs;
 };
 
-static constexpr int kMMDiT = 2;
+static constexpr int kDiT = 0, kUNetT = 1, kMMDiT = 2;  // f5_arch.backbone
 static constexpr int kSkipConcat = 0, kSkipAdd = 1, kSkipNone = 2;  // f5_arch.skip_type (UNetT skip_connect_type)
 
 // MMDiT: first row of block i's modulation vectors in the AdaLN table ([x: 6D | c: 6D] per block, the last block's c
 // part 2D, then norm_out 2D); DiT: [6D] per block, then norm_out
 static size_t mod_block(const f5_arch& A, int i) { return (size_t)i * (A.backbone == kMMDiT ? 12 : 6) * A.dim; }
+
+static void take_stream_bufs(const f5_engine* e, Bump& bp, TokenStream& st) {
+  st.a = bp.take<__half>((size_t)st.rows * e->arch.dim);
+  st.qkv = bp.take<__half>((size_t)st.rows * 3 * e->inner);
+  st.ao = bp.take<__half>((size_t)st.rows * e->inner);
+  st.g = bp.take<__half>((size_t)st.rows * e->arch.ff_inner);
+}
 
 static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int nt, int evals, float cfg,
                         int half = -1) {
@@ -159,16 +176,19 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.packed = (cfg < 1e-5f && half < 0) ? 0 : 1;
   L.Be = (L.packed && half < 0) ? 2 * B : B;
   L.Bx = L.packed ? 2 * B : B;
-  L.seq = A.backbone == 1 ? N + 1 : N;
   L.M = (long long)L.Be * N;
-  L.M1 = (long long)L.Be * L.seq;
-  const int D = A.dim, Td = A.text_dim, F = A.ff_inner;
+  TokenStream& X = L.x;
+  X = TokenStream{};
+  X.seq = A.backbone == kUNetT ? N + 1 : N;
+  X.rows = (long long)L.Be * X.seq;
+  const long long M1 = X.rows;
+  const int D = A.dim, Td = A.text_dim;
   L.step_ptr = bp.take<int>(64);
   L.io = bp.take<SampleIo>(1);
   L.stage = bp.take<OdeStage>(evals);
   L.t_dev = bp.take<float>(evals);
-  L.rope_cos = bp.take<float>((size_t)L.seq * (A.dim_head / 2));
-  L.rope_sin = bp.take<float>((size_t)L.seq * (A.dim_head / 2));
+  X.rope_cos = bp.take<float>((size_t)X.seq * (A.dim_head / 2));
+  X.rope_sin = bp.take<float>((size_t)X.seq * (A.dim_head / 2));
   L.row_len = bp.take<int>(L.Be);
   L.kv_len = bp.take<int>(L.Be);
   L.frame_len = bp.take<int>(L.Be);
@@ -190,47 +210,42 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.h0h = bp.take<__half>((size_t)L.M * D);
   L.c1 = bp.take<__half>((size_t)L.M * D);
   L.skips.clear();
-  if (A.backbone == 1) {
+  if (A.backbone == kUNetT) {
     // concat and add keep the depth/2 saved rows; only concat has the [x | skip] operand of its combiner GEMM
-    L.x = bp.take<float>((size_t)L.M1 * D);
+    X.res = bp.take<float>((size_t)M1 * D);
     if (A.skip_type != kSkipNone)
-      for (int i = 0; i < A.depth / 2; ++i) L.skips.push_back(bp.take<float>((size_t)L.M1 * D));
-    L.cat = A.skip_type == kSkipConcat ? bp.take<__half>((size_t)L.M1 * 2 * D) : nullptr;
+      for (int i = 0; i < A.depth / 2; ++i) L.skips.push_back(bp.take<float>((size_t)M1 * D));
+    L.cat = A.skip_type == kSkipConcat ? bp.take<__half>((size_t)M1 * 2 * D) : nullptr;
   } else {
-    L.x = L.h0;
+    X.res = L.h0;
     L.cat = nullptr;
   }
-  L.a = bp.take<__half>((size_t)L.M1 * D);
-  L.qkv = bp.take<__half>((size_t)L.M1 * 3 * e->inner);
-  L.ao = bp.take<__half>((size_t)L.M1 * e->inner);
-  L.g = bp.take<__half>((size_t)L.M1 * F);
-  L.v_all = bp.take<float>((size_t)L.Bx * L.seq * A.mel_dim);
-  L.v = L.v_all + (half > 0 ? (size_t)B * L.seq * A.mel_dim : 0);
+  take_stream_bufs(e, bp, X);
+  L.v_all = bp.take<float>((size_t)L.Bx * X.seq * A.mel_dim);
+  L.v = L.v_all + (half > 0 ? (size_t)B * X.seq * A.mel_dim : 0);
   // buffers of the architecture options last: with the options off the layout is the one above
   L.x_embed = nullptr;
   if (A.long_skip) {
-    L.x_embed = bp.take<float>((size_t)L.M1 * D);
-    L.cat = bp.take<__half>((size_t)L.M1 * 2 * D);
+    L.x_embed = bp.take<float>((size_t)M1 * D);
+    L.cat = bp.take<__half>((size_t)M1 * 2 * D);
   }
   L.txu = A.text_avg_upsample ? bp.take<float>((size_t)2 * B * N * Td) : nullptr;
-  L.nt = nt;
-  L.c = L.c0 = L.c0_all = nullptr;
-  L.ac = L.qkv_c = L.ao_c = L.g_c = nullptr;
-  L.c_rope_cos = L.c_rope_sin = nullptr;
+  TokenStream& C = L.c;
+  C = TokenStream{};
+  L.c0 = L.c0_all = nullptr;
   L.c_len = L.c_len_all = nullptr;
   if (A.backbone == kMMDiT) {
-    const size_t Mc = (size_t)L.Be * nt;
-    L.c = bp.take<float>(Mc * D);
+    C.seq = nt;
+    C.rows = (long long)L.Be * nt;
+    C.res = bp.take<float>((size_t)C.rows * D);
     L.c0_all = bp.take<float>((size_t)L.Bx * nt * D);
     L.c0 = L.c0_all + (half > 0 ? (size_t)B * nt * D : 0);
-    L.ac = bp.take<__half>(Mc * D);
-    L.qkv_c = bp.take<__half>(Mc * 3 * e->inner);
-    L.ao_c = bp.take<__half>(Mc * e->inner);
-    L.g_c = bp.take<__half>(Mc * F);
-    L.c_rope_cos = bp.take<float>((size_t)nt * (A.dim_head / 2));
-    L.c_rope_sin = bp.take<float>((size_t)nt * (A.dim_head / 2));
+    take_stream_bufs(e, bp, C);
+    C.rope_cos = bp.take<float>((size_t)nt * (A.dim_head / 2));
+    C.rope_sin = bp.take<float>((size_t)nt * (A.dim_head / 2));
     L.c_len_all = bp.take<int>(L.Bx);
     L.c_len = L.c_len_all + (half > 0 ? B : 0);
+    C.out_len = L.c_len;
   }
   L.bytes = bp.off + 512;
 }
@@ -259,7 +274,7 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
     set_error("engine_create: text conv blocks need text_dim %% 64 == 0, <= 512, at most 8 layers");
     return -1;
   }
-  if (arch->backbone < 0 || arch->backbone > kMMDiT) {
+  if (arch->backbone < kDiT || arch->backbone > kMMDiT) {
     set_error("engine_create: backbone must be 0 (DiT), 1 (UNetT) or 2 (MMDiT), got %d", arch->backbone);
     return -1;
   }
@@ -286,7 +301,7 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
       }
     }
   }
-  if ((arch->long_skip || arch->text_avg_upsample) && arch->backbone != 0) {
+  if ((arch->long_skip || arch->text_avg_upsample) && arch->backbone != kDiT) {
     set_error("engine_create: long_skip and text_avg_upsample are DiT options");
     return -1;
   }
@@ -298,12 +313,12 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
     set_error("engine_create: long_skip needs long_skip_w");
     return -1;
   }
-  if (arch->skip_type < kSkipConcat || arch->skip_type > kSkipNone || (arch->skip_type && arch->backbone != 1)) {
+  if (arch->skip_type < kSkipConcat || arch->skip_type > kSkipNone || (arch->skip_type && arch->backbone != kUNetT)) {
     set_error("engine_create: skip_type must be 0 (concat), 1 (add) or 2 (none), and non-zero only for UNetT "
               "(backbone %d, skip_type %d)", arch->backbone, arch->skip_type);
     return -1;
   }
-  if (arch->backbone == 1 && arch->skip_type != kSkipConcat) {
+  if (arch->backbone == kUNetT && arch->skip_type != kSkipConcat) {
     // every first-half layer pushes x and every later-half layer pops one (unett.py:286-294): an odd depth pops more
     // than it pushed
     if (arch->depth % 2) {
@@ -316,7 +331,7 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
         return -1;
       }
   }
-  if (arch->backbone == 1 && arch->skip_type == kSkipConcat)
+  if (arch->backbone == kUNetT && arch->skip_type == kSkipConcat)
     for (int i = arch->depth / 2; i < arch->depth; ++i)
       if (weights->layers[i].w_skip == nullptr) {
         set_error("engine_create: UNetT skip_type concat needs w_skip in every later-half layer (layer %d)", i);
@@ -337,10 +352,16 @@ int f5_engine_create(const f5_arch* arch, const f5_weights* weights, f5_engine**
   e->layers.assign(weights->layers, weights->layers + arch->depth);
   e->w.layers = e->layers.data();
   e->inner = arch->heads * arch->dim_head;
-  e->modW = arch->backbone == 0 ? arch->depth * 6 * arch->dim + 2 * arch->dim : 0;
+  e->modW = arch->backbone == kDiT ? arch->depth * 6 * arch->dim + 2 * arch->dim : 0;
   if (arch->backbone == kMMDiT) {
-    e->ctx.assign(weights->ctx_layers, weights->ctx_layers + arch->depth);
-    e->w.ctx_layers = e->ctx.data();
+    for (int i = 0; i < arch->depth; ++i) {
+      const f5_ctx_layer_weights& c = weights->ctx_layers[i];
+      f5_layer_weights lw{};
+      lw.w_qkv = c.w_qkv_c, lw.b_qkv = c.b_qkv_c, lw.w_out = c.w_out_c, lw.b_out = c.b_out_c;
+      lw.w_ff1 = c.w_ff1_c, lw.b_ff1 = c.b_ff1_c, lw.w_ff2 = c.w_ff2_c, lw.b_ff2 = c.b_ff2_c;
+      lw.q_norm_w = c.q_norm_c, lw.k_norm_w = c.k_norm_c;
+      e->ctx.push_back(lw);
+    }
     e->modW = (int)mod_block(*arch, arch->depth - 1) + 8 * arch->dim + 2 * arch->dim;
   }
   e->kin = weights->proj_kpad;
@@ -370,29 +391,21 @@ size_t f5_sample_workspace_bytes(const f5_engine* e, int B, int N, int nfe, floa
 
 double f5_sample_flops_nt(const f5_engine* e, int B, int N, int nt, int nfe, float cfg_strength) {
   const f5_arch& A = e->arch;
-  if (A.backbone == kMMDiT) {
-    const double D = A.dim, mel = A.mel_dim, F = A.ff_inner, Ld = A.depth, I = e->inner, n = N, m = nt;
-    const double Be = cfg_strength < 1e-5f ? B : 2.0 * B;
-    // every block: audio QKV + out + FF; text QKV; joint attention (QK^T + PV) of the audio queries over N + nt keys.
-    // Every block but the last: text out + FF and the text queries' attention.
-    double per = Ld * (8.0 * n * D * I + 4.0 * n * D * F + 6.0 * m * D * I + 4.0 * n * (n + m) * I) +
-                 (Ld - 1.0) * (2.0 * m * I * D + 4.0 * m * D * F + 4.0 * m * (n + m) * I);
-    per += 2.0 * n * (2 * mel) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n * D * mel;
-    return nfe * Be * per + nfe * (2.0 * 256 * D + 2.0 * D * D + 2.0 * D * (double)e->modW);
-  }
-  return f5_sample_flops(e, B, N, nfe, cfg_strength);
-}
-
-double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
-  const f5_arch& A = e->arch;
-  if (A.backbone == kMMDiT) return f5_sample_flops_nt(e, B, N, N, nfe, cfg_strength);
   const double D = A.dim, mel = A.mel_dim, Td = A.text_dim, F = A.ff_inner, Ld = A.depth;
   // attention width heads * dim_head: QKV 6 n D I + out-projection 2 n I D, QK^T + PV 4 n^2 I.  At dim_head 64 the
-  // count keeps the form it always had (I = D, as in every shipped config), so figures reported before stay comparable.
-  const double I = A.dim_head == 64 ? D : double(e->inner);
+  // DiT / UNetT count keeps the form it always had (I = D, as in every shipped config), so figures reported before stay
+  // comparable.
+  const double I = A.backbone != kMMDiT && A.dim_head == 64 ? D : double(e->inner);
   const double Be = cfg_strength < 1e-5f ? B : 2.0 * B;
   double per;  // one sample-forward
-  if (A.backbone == 0) {
+  if (A.backbone == kMMDiT) {
+    const double n = N, m = nt;
+    // every block: audio QKV + out + FF; text QKV; joint attention (QK^T + PV) of the audio queries over N + nt keys.
+    // Every block but the last: text out + FF and the text queries' attention.
+    per = Ld * (8.0 * n * D * I + 4.0 * n * D * F + 6.0 * m * D * I + 4.0 * n * (n + m) * I) +
+          (Ld - 1.0) * (2.0 * m * I * D + 4.0 * m * D * F + 4.0 * m * (n + m) * I);
+    per += 2.0 * n * (2 * mel) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n * D * mel;
+  } else if (A.backbone == kDiT) {
     const double n = N;
     per = Ld * (8.0 * n * D * I + 4.0 * n * D * F + 4.0 * n * n * I) + 2.0 * n * (2 * mel + Td) * D +
           2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n * D * mel;
@@ -405,11 +418,15 @@ double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_stre
           2.0 * n * (2 * mel + Td) * D + 2.0 * (2.0 * n * D * (D / 16.0) * 31.0) + 2.0 * n1 * D * mel;
   }
   double total = nfe * Be * per;
-  // text embedding, once per sample and CFG branch: conv_layers x (2 pointwise GEMMs)
+  // text embedding, once per sample and CFG branch: conv_layers x (2 pointwise GEMMs); none in MMDiT
   total += 2.0 * B * A.conv_layers * (2.0 * 2.0 * N * Td * 2.0 * Td);
   // conditioning: time MLP + AdaLN table, one row per evaluation, computed once per call
   total += nfe * (2.0 * 256 * D + 2.0 * D * D + 2.0 * D * (double)e->modW);
   return total;
+}
+
+double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength) {
+  return f5_sample_flops_nt(e, B, N, N, nfe, cfg_strength);
 }
 
 }  // extern "C"
@@ -417,10 +434,14 @@ double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_stre
 // -------------------------------------------------------------------------------------------------------------
 namespace {
 
+struct BlockPlans {
+  GemmPlan qkv, oproj, ff1, ff2;
+  GemmPlan skip;  // UNetT later-half layers with skip_type concat: the combiner GEMM
+};
+
 struct StepPlans {
   GemmPlan proj, conv1, conv2, out_proj, long_skip;
-  std::vector<GemmPlan> qkv, oproj, ff1, ff2, skip;
-  std::vector<GemmPlan> qkv_c, oproj_c, ff1_c, ff2_c;  // MMDiT text stream
+  std::vector<BlockPlans> x, c;  // per layer: the audio stream, the MMDiT text stream
   std::vector<AttnPlan> attn;  // identical per layer, kept once (MMDiT: one with text queries, one for the last block)
 };
 
@@ -447,66 +468,72 @@ f5_gemm_args base_args(long long rows, int n_out, int k, int lda, int ldw, int b
 
 constexpr int kAutoTile = 0;  // bn = 0: the GEMM planner picks the tile shape per problem (gemm.cu: pick_tile)
 
-// MMDiT text stream (modules.py:783-846 with context_dim = dim): QKV (+ per-head RMSNorm) + RoPE at text positions
-// 0..nt-1, gated out-projection whose padded rows are zeroed (c_mask, modules.py:700-703), FF pair.  Every text row is
-// computed; the last block has only the QKV.
-int build_text_plans(f5_engine* e, const Layout& L, StepPlans& P) {
+// The four GEMMs of one block of one stream: QKV (+ per-head RMSNorm) + RoPE on the first pe_heads heads, out-projection
+// (+ gate, + zeroed padded rows, + residual), FF1 + GELU, FF2 (+ gate, + residual).  m: the block's AdaLN vectors of
+// this stream (gates at 2D and 5D), or null (UNetT: no gates).  qkv_only: MMDiT's last text block (context_pre_only).
+// The MMDiT text stream (modules.py:783-846 with context_dim = dim) ropes text positions 0..nt-1 on every head, zeroes
+// its padded rows in the out-projection (c_mask, modules.py:700-703) and computes every row.
+int plan_block(const f5_engine* e, const Layout& L, const TokenStream& st, const f5_layer_weights& lw, const float* m,
+               int pe_heads, bool qkv_only, BlockPlans& P) {
   const f5_arch& A = e->arch;
   const int D = A.dim, F = A.ff_inner, inner = e->inner;
-  const long long Mc = (long long)L.Be * L.nt;
-  P.qkv_c.resize(A.depth);
-  P.oproj_c.resize(A.depth);
-  P.ff1_c.resize(A.depth);
-  P.ff2_c.resize(A.depth);
-  for (int i = 0; i < A.depth; ++i) {
-    const f5_ctx_layer_weights& cw = e->w.ctx_layers[i];
-    const float* mc = L.mod + mod_block(A, i) + 6 * D;
-    {
-      f5_gemm_args a = base_args(Mc, 3 * inner, D, D, D, kAutoTile, A.qk_norm ? F5_EPI_QKV_NORM_ROPE : F5_EPI_QKV_ROPE,
-                                 F5_ACT_NONE);
-      a.q_norm = cw.q_norm_c;
-      a.k_norm = cw.k_norm_c;
-      a.bias = cw.b_qkv_c;
-      a.out = L.qkv_c;
-      a.ldo = 3 * inner;
-      a.seq = L.nt;
-      a.rope_cos = L.c_rope_cos;
-      a.rope_sin = L.c_rope_sin;
-      a.inner = inner;
-      a.pe_heads = A.heads;
-      a.dim_head = A.dim_head;
-      RC(gemm_plan(&P.qkv_c[i], L.ac, cw.w_qkv_c, &a));
-    }
-    if (i == A.depth - 1) break;  // context_pre_only
-    {
-      f5_gemm_args a = base_args(Mc, D, inner, inner, inner, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
-      a.bias = cw.b_out_c;
-      a.resid = L.c;
-      a.ldo = D;
-      a.seq = L.nt;
-      a.row_len = L.c_len;
-      a.gate = mc + 2 * D;
-      a.step_ptr = L.step_ptr;
-      a.gate_step_stride = e->modW;
-      RC(gemm_plan(&P.oproj_c[i], L.ao_c, cw.w_out_c, &a));
-    }
-    {
-      f5_gemm_args a = base_args(Mc, F, D, D, D, kAutoTile, F5_EPI_F16, F5_ACT_GELU_TANH);
-      a.bias = cw.b_ff1_c;
-      a.out = L.g_c;
-      a.ldo = F;
-      RC(gemm_plan(&P.ff1_c[i], L.ac, cw.w_ff1_c, &a));
-    }
-    {
-      f5_gemm_args a = base_args(Mc, D, F, F, F, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
-      a.bias = cw.b_ff2_c;
-      a.resid = L.c;
-      a.ldo = D;
-      a.gate = mc + 5 * D;
-      a.step_ptr = L.step_ptr;
-      a.gate_step_stride = e->modW;
-      RC(gemm_plan(&P.ff2_c[i], L.g_c, cw.w_ff2_c, &a));
-    }
+  auto varlen = [&](f5_gemm_args& a) {
+    if (!st.skip_len) return;
+    a.row_len = st.skip_len;
+    a.seq = st.seq;
+    a.skip_padded_tiles = 1;
+  };
+  auto gate = [&](f5_gemm_args& a, int off) {
+    if (!m) return;
+    a.gate = m + off * D;
+    a.step_ptr = L.step_ptr;
+    a.gate_step_stride = e->modW;
+  };
+  {
+    f5_gemm_args a = base_args(st.rows, 3 * inner, D, D, D, kAutoTile, A.qk_norm ? F5_EPI_QKV_NORM_ROPE : F5_EPI_QKV_ROPE,
+                               F5_ACT_NONE);
+    a.q_norm = lw.q_norm_w;
+    a.k_norm = lw.k_norm_w;
+    a.bias = lw.b_qkv;
+    a.out = st.qkv;
+    a.ldo = 3 * inner;
+    a.seq = st.seq;
+    a.rope_cos = st.rope_cos;
+    a.rope_sin = st.rope_sin;
+    a.inner = inner;
+    a.pe_heads = pe_heads;
+    a.dim_head = A.dim_head;
+    varlen(a);
+    RC(gemm_plan(&P.qkv, st.a, lw.w_qkv, &a));
+  }
+  if (qkv_only) return 0;
+  {
+    f5_gemm_args a = base_args(st.rows, D, inner, inner, inner, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
+    a.bias = lw.b_out;
+    a.resid = st.res;
+    a.ldo = D;
+    a.seq = st.seq;
+    a.row_len = st.out_len;
+    gate(a, 2);
+    varlen(a);
+    RC(gemm_plan(&P.oproj, st.ao, lw.w_out, &a));
+  }
+  {
+    f5_gemm_args a = base_args(st.rows, F, D, D, D, kAutoTile, F5_EPI_F16, F5_ACT_GELU_TANH);
+    a.bias = lw.b_ff1;
+    a.out = st.g;
+    a.ldo = F;
+    varlen(a);
+    RC(gemm_plan(&P.ff1, st.a, lw.w_ff1, &a));
+  }
+  {
+    f5_gemm_args a = base_args(st.rows, D, F, F, F, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
+    a.bias = lw.b_ff2;
+    a.resid = st.res;
+    a.ldo = D;
+    gate(a, 5);
+    varlen(a);
+    RC(gemm_plan(&P.ff2, st.g, lw.w_ff2, &a));
   }
   return 0;
 }
@@ -514,17 +541,14 @@ int build_text_plans(f5_engine* e, const Layout& L, StepPlans& P) {
 int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, StepPlans& P) {
   const f5_arch& A = e->arch;
   const f5_weights& W = e->w;
-  const int D = A.dim, F = A.ff_inner, inner = e->inner;
-  const bool dit = A.backbone == 0;
+  const int D = A.dim;
+  const long long M1 = L.x.rows;
   const bool mmdit = A.backbone == kMMDiT;
-  const bool adaln = A.backbone != 1;  // DiT and MMDiT: AdaLN modulation from the per-call table
   const bool masked = sa->duration != nullptr;
   const bool strict = masked && sa->exact_varlen;  // every sample exactly as if alone in the batch (f5_sample_args)
   // input projection / conv position embedding see per-sample lengths (MMDiT's AudioEmbedding takes no mask,
   // backbones/mmdit.py:67-78: only exact_varlen confines it)
-  const bool mask_in = (dit && masked) || strict;
-  const int pe_heads = A.pe_attn_head < 0 ? A.heads : A.pe_attn_head;
-  const long long modS = e->modW;
+  const bool mask_in = (A.backbone == kDiT && masked) || strict;
 
   {  // input projection: h0 = xin . proj_w^T + b ; h0h = fp16(mask(h0))
     f5_gemm_args a = base_args(L.M, D, e->kin, e->kin, e->kin, 128, F5_EPI_F32, F5_ACT_NONE);
@@ -562,12 +586,6 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
       RC(gemm_plan(&P.conv2, L.c1, W.conv_w[1], &a));
     }
   }
-  P.qkv.resize(A.depth);
-  P.oproj.resize(A.depth);
-  P.ff1.resize(A.depth);
-  P.ff2.resize(A.depth);
-  P.skip.resize(A.depth);
-  const int* rl = masked ? L.row_len : nullptr;
   // Variable-length execution (SURVEY.md §8f-1): in the reference's key-masked mode (attn_mask_enabled, modules.py:
   // 513-518) padded rows influence nothing, so every GEMM / conv / attention tile that holds only padding is skipped.
   // In the default "faithful" mode padded keys ARE attended (SURVEY.md §0.5) and every row must be computed.
@@ -575,101 +593,51 @@ int build_step_plans(f5_engine* e, const Layout& L, const f5_sample_args* sa, St
   // MMDiT's conv position embedding reads padded audio rows (no mask, mmdit.py:67-78), and those rows evolve with the
   // ODE like any other: outside exact_varlen they must be computed in full.  UNetT's conv is unmasked too
   // (unett.py:90-102); add and none compute every row the same way, concat keeps the tile skipping it always had.
-  const bool unmasked_conv = mmdit || (A.backbone == 1 && A.skip_type != kSkipConcat);
+  const bool unmasked_conv = mmdit || (A.backbone == kUNetT && A.skip_type != kSkipConcat);
   const int skip = unmasked_conv ? (strict ? 1 : 0) : key_mask;
-  auto varlen = [&](f5_gemm_args& a) {
-    if (!skip) return;
-    a.row_len = L.row_len;
-    a.seq = L.seq;
-    a.skip_padded_tiles = 1;
-  };
+  TokenStream X = L.x;
+  X.out_len = masked ? L.row_len : nullptr;
+  X.skip_len = skip ? L.row_len : nullptr;
+  const int pe_heads = A.pe_attn_head < 0 ? A.heads : A.pe_attn_head;
+  P.x.resize(A.depth);
   for (int i = 0; i < A.depth; ++i) {
-    const f5_layer_weights& lw = W.layers[i];
-    if (!dit && lw.w_skip) {
-      f5_gemm_args a = base_args(L.M1, D, 2 * D, 2 * D, 2 * D, 128, F5_EPI_F32, F5_ACT_NONE);
-      a.out = L.x;
+    const f5_layer_weights& lw = e->layers[i];
+    if (A.backbone != kDiT && lw.w_skip) {
+      f5_gemm_args a = base_args(M1, D, 2 * D, 2 * D, 2 * D, 128, F5_EPI_F32, F5_ACT_NONE);
+      a.out = X.res;
       a.ldo = D;
-      RC(gemm_plan(&P.skip[i], L.cat, lw.w_skip, &a));  // (EPI_F32 direct-store path: not tile-skipped)
+      RC(gemm_plan(&P.x[i].skip, L.cat, lw.w_skip, &a));  // (EPI_F32 direct-store path: not tile-skipped)
     }
-    {
-      f5_gemm_args a = base_args(L.M1, 3 * inner, D, D, D, kAutoTile, A.qk_norm ? F5_EPI_QKV_NORM_ROPE : F5_EPI_QKV_ROPE,
-                                 F5_ACT_NONE);
-      a.q_norm = lw.q_norm_w;
-      a.k_norm = lw.k_norm_w;
-      a.bias = lw.b_qkv;
-      a.out = L.qkv;
-      a.ldo = 3 * inner;
-      a.seq = L.seq;
-      a.rope_cos = L.rope_cos;
-      a.rope_sin = L.rope_sin;
-      a.inner = inner;
-      a.pe_heads = pe_heads;
-      a.dim_head = A.dim_head;
-      varlen(a);
-      RC(gemm_plan(&P.qkv[i], L.a, lw.w_qkv, &a));
-    }
-    {
-      f5_gemm_args a = base_args(L.M1, D, inner, inner, inner, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
-      a.bias = lw.b_out;
-      a.resid = L.x;
-      a.ldo = D;
-      a.seq = L.seq;
-      a.row_len = rl;
-      if (adaln) {
-        a.gate = L.mod + mod_block(A, i) + 2 * D;
-        a.step_ptr = L.step_ptr;
-        a.gate_step_stride = modS;
-      }
-      varlen(a);
-      RC(gemm_plan(&P.oproj[i], L.ao, lw.w_out, &a));
-    }
-    {
-      f5_gemm_args a = base_args(L.M1, F, D, D, D, kAutoTile, F5_EPI_F16, F5_ACT_GELU_TANH);
-      a.bias = lw.b_ff1;
-      a.out = L.g;
-      a.ldo = F;
-      varlen(a);
-      RC(gemm_plan(&P.ff1[i], L.a, lw.w_ff1, &a));
-    }
-    {
-      f5_gemm_args a = base_args(L.M1, D, F, F, F, kAutoTile, F5_EPI_RESID, F5_ACT_NONE);
-      a.bias = lw.b_ff2;
-      a.resid = L.x;
-      a.ldo = D;
-      if (adaln) {
-        a.gate = L.mod + mod_block(A, i) + 5 * D;
-        a.step_ptr = L.step_ptr;
-        a.gate_step_stride = modS;
-      }
-      varlen(a);
-      RC(gemm_plan(&P.ff2[i], L.g, lw.w_ff2, &a));
-    }
+    const float* m = A.backbone == kUNetT ? nullptr : L.mod + mod_block(A, i);  // DiT and MMDiT: AdaLN gates
+    RC(plan_block(e, L, X, lw, m, pe_heads, false, P.x[i]));
   }
   if (A.long_skip) {  // x = cat(x, x_embed) . long_skip_w^T, no bias (backbones/dit.py:228, 363-364)
-    f5_gemm_args a = base_args(L.M1, D, 2 * D, 2 * D, 2 * D, 128, F5_EPI_F32, F5_ACT_NONE);
-    a.out = L.x;
+    f5_gemm_args a = base_args(M1, D, 2 * D, 2 * D, 2 * D, 128, F5_EPI_F32, F5_ACT_NONE);
+    a.out = X.res;
     a.ldo = D;
     RC(gemm_plan(&P.long_skip, L.cat, W.long_skip_w, &a));
   }
   {
-    f5_gemm_args a = base_args(L.M1, A.mel_dim, D, D, D, 128, F5_EPI_F32, F5_ACT_NONE);
+    f5_gemm_args a = base_args(M1, A.mel_dim, D, D, D, 128, F5_EPI_F32, F5_ACT_NONE);
     a.bias = W.out_b;
     a.out = L.v;
     a.ldo = A.mel_dim;
-    RC(gemm_plan(&P.out_proj, L.a, W.out_w, &a));
+    RC(gemm_plan(&P.out_proj, X.a, W.out_w, &a));
   }
   P.attn.resize(1);
   if (mmdit) {
-    RC(build_text_plans(e, L, P));
+    P.c.resize(A.depth);
+    for (int i = 0; i < A.depth; ++i)
+      RC(plan_block(e, L, L.c, e->ctx[i], L.mod + mod_block(A, i) + 6 * D, A.heads, i == A.depth - 1, P.c[i]));
     // joint attention: [0] for the blocks with text queries, [1] for the last block, whose text output is discarded
     P.attn.resize(2);
     for (int last = 0; last < 2; ++last)
-      RC(attn_joint_plan(&P.attn[last], L.qkv, L.qkv_c, L.ao, L.ao_c, L.Be, L.seq, L.nt, A.heads, A.dim_head,
+      RC(attn_joint_plan(&P.attn[last], X.qkv, L.c.qkv, X.ao, L.c.ao, L.Be, X.seq, L.c.seq, A.heads, A.dim_head,
                          key_mask ? L.kv_len : nullptr, key_mask ? L.c_len : nullptr, last ? 0 : 1,
                          1.0f / sqrtf((float)A.dim_head)));
     return 0;
   }
-  RC(attn_plan(&P.attn[0], L.qkv, L.ao, L.Be, L.seq, A.heads, A.dim_head, key_mask ? L.kv_len : nullptr,
+  RC(attn_plan(&P.attn[0], X.qkv, X.ao, L.Be, X.seq, A.heads, A.dim_head, key_mask ? L.kv_len : nullptr,
                1.0f / sqrtf((float)A.dim_head)));
   return 0;
 }
@@ -685,13 +653,13 @@ static bool diag_skip(const char* what) {
 static constexpr bool diag_skip(const char*) { return false; }
 #endif
 
-int norm_mod(const f5_engine* e, const Layout& L, const float* x, long long rows, int mode, const float* a,
-             const float* b, bool step_indexed, cudaStream_t s, __half* out = nullptr, const float* skip = nullptr) {
+int norm_mod(const f5_engine* e, const Layout& L, const TokenStream& st, int mode, const float* a, const float* b,
+             bool step_indexed, cudaStream_t s, const float* skip = nullptr) {
   NormParams p{};
   p.skip = skip;
-  p.x = x;
-  p.out = out ? out : L.a;
-  p.rows = (int)rows;
+  p.x = st.res;
+  p.out = st.a;
+  p.rows = (int)st.rows;
   p.D = e->arch.dim;
   p.eps = 1e-6f;
   p.a = a;
@@ -703,100 +671,86 @@ int norm_mod(const f5_engine* e, const Layout& L, const float* x, long long rows
   return run_row_norm(mode, p, s);
 }
 
-// One MMDiT block (modules.py:806-846): both streams' AdaLN, QKV, joint attention, gated out-projections and FF pairs
-int run_mmdit_block(f5_engine* e, const Layout& L, const StepPlans& P, int i, cudaStream_t s) {
+int gemm_step(const GemmPlan& plan, const char* what, cudaStream_t s) {
+  return diag_skip(what) ? 0 : gemm_run(plan, s);
+}
+
+// Norm -> FF1 -> FF2 of one stream: AdaLN with the block's vectors m (scale_mlp, shift_mlp), or, m null, UNetT's
+// RMSNorm with gain g
+int run_ff(const f5_engine* e, const Layout& L, const TokenStream& st, const BlockPlans& bp, const float* m,
+           const float* g, cudaStream_t s) {
+  const int D = e->arch.dim;
+  RC(m ? norm_mod(e, L, st, 0, m + 4 * D, m + 3 * D, true, s) : norm_mod(e, L, st, 2, g, nullptr, false, s));
+  RC(gemm_step(bp.ff1, "ff1", s));
+  return gemm_step(bp.ff2, "ff2", s);
+}
+
+// One transformer block.  MMDiT (modules.py:806-846) runs the text stream beside the audio stream: both streams' AdaLN
+// and QKV, one joint attention, then the text stream's gated out-projection and FF pair before the audio stream's FF
+// pair (the last block computes only the text QKV).
+int run_block(f5_engine* e, const Layout& L, const StepPlans& P, int i, cudaStream_t s) {
   const f5_arch& A = e->arch;
   const int D = A.dim;
-  const bool last = i == A.depth - 1;
-  const long long Mc = (long long)L.Be * L.nt;
-  const float* mx = L.mod + mod_block(A, i);
-  const float* mc = mx + 6 * D;
-  RC(norm_mod(e, L, L.x, L.M1, 0, mx + D, mx, true, s));  // attn_norm_x: scale_msa, shift_msa
-  if (last)
-    RC(norm_mod(e, L, L.c, Mc, 0, mc, mc + D, true, s, L.ac));  // AdaLayerNorm_Final: scale, shift
-  else
-    RC(norm_mod(e, L, L.c, Mc, 0, mc + D, mc, true, s, L.ac));
-  RC(gemm_run(P.qkv[i], s));
-  RC(gemm_run(P.qkv_c[i], s));
-  RC(attn_run(P.attn[last ? 1 : 0], s));
-  RC(gemm_run(P.oproj[i], s));
-  if (!last) {
-    RC(gemm_run(P.oproj_c[i], s));
-    RC(norm_mod(e, L, L.c, Mc, 0, mc + 4 * D, mc + 3 * D, true, s, L.ac));  // ff_norm_c: c_scale_mlp, c_shift_mlp
-    RC(gemm_run(P.ff1_c[i], s));
-    RC(gemm_run(P.ff2_c[i], s));
+  const bool mmdit = A.backbone == kMMDiT, last = i == A.depth - 1;
+  const f5_layer_weights& lw = e->layers[i];
+  const float* mx = A.backbone == kUNetT ? nullptr : L.mod + mod_block(A, i);
+  const float* mc = mmdit ? mx + 6 * D : nullptr;
+  if (mx) {
+    RC(norm_mod(e, L, L.x, 0, mx + D, mx, true, s));  // scale_msa, shift_msa
+  } else if (A.skip_type == kSkipAdd && i >= A.depth / 2) {
+    // x += skip and attn_norm in one pass over the rows (row norm mode 3)
+    RC(norm_mod(e, L, L.x, 3, lw.g_attn, nullptr, false, s, L.skips[A.depth - 1 - i]));
+  } else {
+    if (A.skip_type != kSkipNone && i < A.depth / 2) {
+      RC(check_cuda(cudaMemcpyAsync(L.skips[i], L.x.res, sizeof(float) * L.x.rows * D, cudaMemcpyDeviceToDevice, s),
+                    "skip copy"));
+    } else if (A.skip_type == kSkipConcat) {
+      RC(run_concat_half(L.x.res, L.skips[A.depth - 1 - i], L.cat, L.x.rows, D, s));
+      RC(gemm_run(P.x[i].skip, s));
+    }
+    RC(norm_mod(e, L, L.x, 2, lw.g_attn, nullptr, false, s));
   }
-  RC(norm_mod(e, L, L.x, L.M1, 0, mx + 4 * D, mx + 3 * D, true, s));  // ff_norm_x: scale_mlp, shift_mlp
-  RC(gemm_run(P.ff1[i], s));
-  return gemm_run(P.ff2[i], s);
+  if (mmdit)  // last: AdaLayerNorm_Final (scale, shift)
+    RC(last ? norm_mod(e, L, L.c, 0, mc, mc + D, true, s) : norm_mod(e, L, L.c, 0, mc + D, mc, true, s));
+  RC(gemm_step(P.x[i].qkv, "qkv", s));
+  if (mmdit) RC(gemm_step(P.c[i].qkv, "qkv", s));
+  if (!diag_skip("attn")) RC(attn_run(P.attn[mmdit && last ? 1 : 0], s));
+  RC(gemm_step(P.x[i].oproj, "out", s));
+  if (mmdit && !last) {
+    RC(gemm_step(P.c[i].oproj, "out", s));
+    RC(run_ff(e, L, L.c, P.c[i], mc, nullptr, s));
+  }
+  return run_ff(e, L, L.x, P.x[i], mx, lw.g_ff, s);
 }
 
 // One backbone evaluation up to and including proj_out: v (this layout's half of it when split) holds the flow
 int run_body(f5_engine* e, const Layout& L, const StepPlans& P, cudaStream_t s) {
   const f5_arch& A = e->arch;
   const int D = A.dim;
-  const bool dit = A.backbone == 0;
-  const bool mmdit = A.backbone == kMMDiT;
   RC(gemm_run(P.proj, s));
   if (!diag_skip("conv")) {
     RC(gemm_run(P.conv1, s));
     RC(gemm_run(P.conv2, s));
   }
-  if (A.backbone == 1) RC(run_prepend_time_token(L.x, L.h0, L.temb, L.step_ptr, L.N, D, L.M1, s));
-  if (mmdit) {
+  if (A.backbone == kUNetT) RC(run_prepend_time_token(L.x.res, L.h0, L.temb, L.step_ptr, L.N, D, L.x.rows, s));
+  if (A.backbone == kMMDiT) {
     // the text stream restarts from its embedding at every evaluation (get_input_embed, mmdit.py:177-196)
-    RC(check_cuda(cudaMemcpyAsync(L.c, L.c0, sizeof(float) * L.Be * L.nt * D,
-                                  cudaMemcpyDeviceToDevice, s), "text stream copy"));
+    RC(check_cuda(cudaMemcpyAsync(L.c.res, L.c0, sizeof(float) * L.c.rows * D, cudaMemcpyDeviceToDevice, s),
+                  "text stream copy"));
   }
   if (A.long_skip)
-    RC(check_cuda(cudaMemcpyAsync(L.x_embed, L.x, sizeof(float) * L.M1 * D, cudaMemcpyDeviceToDevice, s),
+    RC(check_cuda(cudaMemcpyAsync(L.x_embed, L.x.res, sizeof(float) * L.x.rows * D, cudaMemcpyDeviceToDevice, s),
                   "long skip copy"));
-  const int half = A.depth / 2;
-  for (int i = 0; i < A.depth; ++i) {
-    if (mmdit) {
-      RC(run_mmdit_block(e, L, P, i, s));
-      continue;
-    }
-    const f5_layer_weights& lw = e->w.layers[i];
-    if (dit) {
-      const float* m = L.mod + (size_t)i * 6 * D;
-      RC(norm_mod(e, L, L.x, L.M1, 0, m + D, m, true, s));  // scale_msa, shift_msa
-    } else {
-      if (A.skip_type == kSkipAdd && i >= half) {
-        // x += skip and attn_norm in one pass over the rows (row norm mode 3)
-        RC(norm_mod(e, L, L.x, L.M1, 3, lw.g_attn, nullptr, false, s, nullptr, L.skips[A.depth - 1 - i]));
-      } else {
-        if (A.skip_type != kSkipNone && i < half) {
-          RC(check_cuda(cudaMemcpyAsync(L.skips[i], L.x, sizeof(float) * L.M1 * D, cudaMemcpyDeviceToDevice, s),
-                        "skip copy"));
-        } else if (A.skip_type == kSkipConcat) {
-          RC(run_concat_half(L.x, L.skips[A.depth - 1 - i], L.cat, L.M1, D, s));
-          RC(gemm_run(P.skip[i], s));
-        }
-        RC(norm_mod(e, L, L.x, L.M1, 2, lw.g_attn, nullptr, false, s));
-      }
-    }
-    if (!diag_skip("qkv")) RC(gemm_run(P.qkv[i], s));
-    if (!diag_skip("attn")) RC(attn_run(P.attn[0], s));
-    if (!diag_skip("out")) RC(gemm_run(P.oproj[i], s));
-    if (dit) {
-      const float* m = L.mod + (size_t)i * 6 * D;
-      RC(norm_mod(e, L, L.x, L.M1, 0, m + 4 * D, m + 3 * D, true, s));  // scale_mlp, shift_mlp
-    } else {
-      RC(norm_mod(e, L, L.x, L.M1, 2, lw.g_ff, nullptr, false, s));
-    }
-    if (!diag_skip("ff1")) RC(gemm_run(P.ff1[i], s));
-    if (!diag_skip("ff2")) RC(gemm_run(P.ff2[i], s));
-  }
+  for (int i = 0; i < A.depth; ++i) RC(run_block(e, L, P, i, s));
   if (A.long_skip) {
-    RC(run_concat_half(L.x, L.x_embed, L.cat, L.M1, D, s));
+    RC(run_concat_half(L.x.res, L.x_embed, L.cat, L.x.rows, D, s));
     RC(gemm_run(P.long_skip, s));
   }
-  if (dit || mmdit) {
-    const float* m = L.mod + (e->modW - 2 * D);
-    RC(norm_mod(e, L, L.x, L.M1, 0, m, m + D, true, s));  // AdaLayerNorm_Final: scale, shift (modules.py:342-347)
+  if (A.backbone == kUNetT) {
+    RC(norm_mod(e, L, L.x, 2, e->w.g_out, nullptr, false, s));
   } else {
-    RC(norm_mod(e, L, L.x, L.M1, 2, e->w.g_out, nullptr, false, s));
+    const float* m = L.mod + (e->modW - 2 * D);
+    RC(norm_mod(e, L, L.x, 0, m, m + D, true, s));  // AdaLayerNorm_Final: scale, shift (modules.py:342-347)
   }
   return gemm_run(P.out_proj, s);
 }
@@ -815,8 +769,8 @@ int run_update(const f5_engine* e, const Layout& L, cudaStream_t s) {
   ep.Kpad = e->kin;
   ep.packed = L.packed;
   ep.N = L.N;
-  ep.seq_tok = L.seq;
-  ep.tok_off = A.backbone == 1 ? 1 : 0;
+  ep.seq_tok = L.x.seq;
+  ep.tok_off = A.backbone == kUNetT ? 1 : 0;
   ep.B = L.B;
   return run_cfg_euler(ep, s);
 }
@@ -830,7 +784,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   const f5_arch& A = e->arch;
   const f5_weights& W = e->w;
   const int D = A.dim, Td = A.text_dim, B = L.B, N = L.N, S = L.evals;
-  const bool dit = A.backbone == 0;
+  const bool dit = A.backbone == kDiT;
   const bool mmdit = A.backbone == kMMDiT;
   const bool masked = sa->duration != nullptr;
   const bool strict = masked && sa->exact_varlen;
@@ -866,7 +820,7 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     RC(check_cuda(cudaMemcpyAsync(hd.data(), sa->duration, sizeof(int) * B, cudaMemcpyDeviceToHost, s), "dur d2h"));
     RC(check_cuda(cudaStreamSynchronize(s), "dur sync"));
     std::vector<int> rl(L.Be);
-    for (int i = 0; i < L.Be; ++i) rl[i] = hd[i % B] + (A.backbone == 1 ? 1 : 0);
+    for (int i = 0; i < L.Be; ++i) rl[i] = hd[i % B] + (A.backbone == kUNetT ? 1 : 0);
     RC(check_cuda(cudaMemcpyAsync(L.row_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "row_len"));
     RC(check_cuda(cudaMemcpyAsync(L.kv_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "kv_len"));
     RC(check_cuda(cudaMemcpyAsync(L.valid_len, hd.data(), sizeof(int) * B, cudaMemcpyHostToDevice, s), "valid_len"));
@@ -879,10 +833,10 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
       // zero there (= the conv's padding), and q/k/v rows next to a sample's end are multiplied by P = 0 (must be finite)
       RC(check_cuda(cudaMemsetAsync(L.h0h, 0, sizeof(__half) * L.M * D, s), "h0h clear"));
       RC(check_cuda(cudaMemsetAsync(L.c1, 0, sizeof(__half) * L.M * D, s), "c1 clear"));
-      RC(check_cuda(cudaMemsetAsync(L.qkv, 0, sizeof(__half) * L.M1 * 3 * e->inner, s), "qkv clear"));
+      RC(check_cuda(cudaMemsetAsync(L.x.qkv, 0, sizeof(__half) * L.x.rows * 3 * e->inner, s), "qkv clear"));
     }
   }
-  RC(run_rope_table(L.rope_cos, L.rope_sin, L.seq, A.dim_head / 2, s));
+  RC(run_rope_table(L.x.rope_cos, L.x.rope_sin, L.x.seq, A.dim_head / 2, s));
   // time embedding for every evaluation time (modules.py:852-862)
   RC(run_time_features(L.t_dev, L.tfeat, S, 256, s));
   RC(run_small_linear(1, L.tfeat, reinterpret_cast<const __half*>(W.time_w0), W.time_b0, L.th1, S, 256, D, s));
@@ -898,9 +852,9 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     RC(gemm_run(pl, s));
   }
   if (mmdit) {  // text embedding of both CFG variants and the text rope table; no text columns in the input projection
-    RC(run_mmdit_text_embed(sa->text, B, L.Bx, L.nt, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding,
+    RC(run_mmdit_text_embed(sa->text, B, L.Bx, L.c.seq, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding,
                             L.c0_all, L.c_len_all, s));
-    RC(run_rope_table(L.c_rope_cos, L.c_rope_sin, L.nt, A.dim_head / 2, s));
+    RC(run_rope_table(L.c.rope_cos, L.c.rope_sin, L.c.seq, A.dim_head / 2, s));
   }
   // text embedding, both CFG variants (dit.py:86-139 / unett.py:55-84)
   TextGatherParams tp{};
@@ -971,9 +925,9 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
 int copy_v_out(const f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaStream_t s) {
   if (!sa->v_out) return 0;
   const int mel = e->arch.mel_dim;
-  const int off = e->arch.backbone == 1 ? 1 : 0;
+  const int off = e->arch.backbone == kUNetT ? 1 : 0;
   for (int b = 0; b < L.Bx; ++b)
-    RC(check_cuda(cudaMemcpyAsync(sa->v_out + (size_t)b * L.N * mel, L.v_all + ((size_t)b * L.seq + off) * mel,
+    RC(check_cuda(cudaMemcpyAsync(sa->v_out + (size_t)b * L.N * mel, L.v_all + ((size_t)b * L.x.seq + off) * mel,
                                   sizeof(float) * L.N * mel, cudaMemcpyDeviceToDevice, s),
                   "v_out copy"));
   return 0;
@@ -1041,34 +995,59 @@ int check_problem(const char* fn, const f5_sample_args* sa) {
   return 0;
 }
 
+// One side of a call: the whole call of f5_sample, or one CFG half of f5_sample_cfg_split (below)
+struct Side {
+  f5_engine* e;
+  const f5_sample_args* sa;
+  void* ws;
+  size_t bytes;
+  cudaStream_t s;
+  int dev = -1;
+  Layout L;
+  StepPlans P;                      // without use_graph
+  std::shared_ptr<GraphHolder> g;  // with use_graph
+  cudaEvent_t ready = nullptr, pulled = nullptr;  // CFG split only
+};
+
+// The workspace layout of one side (half -1: f5_sample; 0 / 1: that CFG half) and the check that it fits
+int side_layout(Side& sd, int half) {
+  const f5_sample_args* sa = sd.sa;
+  const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
+  plan_layout(sd.e, sd.L, sd.ws, sa->B, sa->N, sa->nt, evals, sa->cfg_strength, half);
+  if (sd.bytes >= sd.L.bytes) return 0;
+  if (half < 0)
+    set_error("f5_sample: workspace too small (%zu < %zu)", sd.bytes, sd.L.bytes);
+  else
+    set_error("f5_sample_cfg_split: workspace %d too small (%zu < %zu)", half, sd.bytes, sd.L.bytes);
+  return -1;
+}
+
+// The prologue of one side, then its step graph (use_graph) or its plans
+int side_prepare(Side& sd) {
+  RC(run_prologue(sd.e, sd.L, sd.sa, sd.s));
+  if (sd.sa->use_graph) return step_graph(sd.e, sd.L, sd.sa, sd.ws, &sd.g);
+  return build_step_plans(sd.e, sd.L, sd.sa, sd.P);
+}
+
 }  // namespace
 
 extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace, size_t ws_bytes, f5_stream_t stream) {
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   if (!e || !sa || !workspace) {
     set_error("f5_sample: null argument");
     return -1;
   }
   RC(check_problem("f5_sample", sa));
-  const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
-  Layout L;
-  plan_layout(e, L, workspace, sa->B, sa->N, sa->nt, evals, sa->cfg_strength);
-  if (ws_bytes < L.bytes) {
-    set_error("f5_sample: workspace too small (%zu < %zu)", ws_bytes, L.bytes);
-    return -1;
+  Side sd{e, sa, workspace, ws_bytes, reinterpret_cast<cudaStream_t>(stream)};
+  RC(side_layout(sd, -1));
+  RC(side_prepare(sd));
+  const int evals = sd.L.evals;
+  if (sd.g) {
+    for (int k = 0; k < evals; ++k) RC(check_cuda(cudaGraphLaunch(sd.g->exec, sd.s), "graph launch"));
+    count_launch(sd.g->nodes * evals);
+  } else {
+    for (int k = 0; k < evals; ++k) RC(run_step(e, sd.L, sd.P, sd.s));
   }
-  RC(run_prologue(e, L, sa, s));
-  if (sa->use_graph) {
-    std::shared_ptr<GraphHolder> g;
-    RC(step_graph(e, L, sa, workspace, &g));
-    for (int k = 0; k < evals; ++k) RC(check_cuda(cudaGraphLaunch(g->exec, s), "graph launch"));
-    count_launch(g->nodes * evals);
-    return copy_v_out(e, L, sa, s);
-  }
-  StepPlans P;
-  RC(build_step_plans(e, L, sa, P));
-  for (int k = 0; k < evals; ++k) RC(run_step(e, L, P, s));
-  return copy_v_out(e, L, sa, s);
+  return copy_v_out(e, sd.L, sa, sd.s);
 }
 
 // -------------------------------------------------------------------------------------------------------------
@@ -1094,19 +1073,6 @@ extern "C" int f5_sample(f5_engine* e, const f5_sample_args* sa, void* workspace
 // issued: if a side fails partway and the host stops, a wait on an event whose record was never issued refers to the
 // previous record or none, and does not block.  No kernel waits on a flag written by the other side.
 namespace {
-
-struct SplitSide {
-  f5_engine* e;
-  const f5_sample_args* sa;
-  void* ws;
-  size_t bytes;
-  cudaStream_t s;
-  int dev = -1;
-  Layout L;
-  StepPlans P;
-  std::shared_ptr<GraphHolder> g;
-  cudaEvent_t ready = nullptr, pulled = nullptr;
-};
 
 int pointer_device(const void* p, const char* what, int* dev) {
   cudaPointerAttributes at{};
@@ -1141,7 +1107,7 @@ int enable_peer_access(int dev, int peer) {
   return 0;
 }
 
-int split_check(const SplitSide* sd) {
+int split_check(const Side* sd) {
   const f5_sample_args *a = sd[0].sa, *b = sd[1].sa;
   if (a->B != b->B || a->N != b->N || a->nt != b->nt || a->steps != b->steps || a->method != b->method ||
       a->use_graph != b->use_graph || a->exact_varlen != b->exact_varlen || a->cfg_strength != b->cfg_strength ||
@@ -1179,11 +1145,11 @@ int split_check(const SplitSide* sd) {
   return 0;
 }
 
-int split_loop(SplitSide* sd, int evals) {
-  const size_t half_floats = (size_t)sd[0].L.B * sd[0].L.seq * sd[0].e->arch.mel_dim;
+int split_loop(Side* sd, int evals) {
+  const size_t half_floats = (size_t)sd[0].L.B * sd[0].L.x.seq * sd[0].e->arch.mel_dim;
   for (int k = 0; k < evals; ++k) {
     for (int d = 0; d < 2; ++d) {
-      SplitSide &me = sd[d], &o = sd[1 - d];
+      Side &me = sd[d], &o = sd[1 - d];
       RC(check_cuda(cudaSetDevice(me.dev), "cudaSetDevice"));
       if (k > 0) RC(check_cuda(cudaStreamWaitEvent(me.s, o.pulled, 0), "wait pulled"));
       if (me.g) {
@@ -1195,7 +1161,7 @@ int split_loop(SplitSide* sd, int evals) {
       RC(check_cuda(cudaEventRecord(me.ready, me.s), "record ready"));
     }
     for (int d = 0; d < 2; ++d) {
-      SplitSide &me = sd[d], &o = sd[1 - d];
+      Side &me = sd[d], &o = sd[1 - d];
       RC(check_cuda(cudaSetDevice(me.dev), "cudaSetDevice"));
       RC(check_cuda(cudaStreamWaitEvent(me.s, o.ready, 0), "wait ready"));
       RC(check_cuda(cudaMemcpyPeerAsync(me.L.v_all + (o.L.v - o.L.v_all), me.dev, o.L.v, o.dev,
@@ -1208,33 +1174,20 @@ int split_loop(SplitSide* sd, int evals) {
   return 0;
 }
 
-int split_run(SplitSide* sd) {
-  const f5_sample_args* sa = sd[0].sa;
-  const int evals = sa->method == 1 ? 2 * sa->steps : sa->steps;
-  for (int d = 0; d < 2; ++d) {
-    SplitSide& me = sd[d];
-    plan_layout(me.e, me.L, me.ws, sa->B, sa->N, sa->nt, evals, sa->cfg_strength, d);
-    if (me.bytes < me.L.bytes) {
-      set_error("f5_sample_cfg_split: workspace %d too small (%zu < %zu)", d, me.bytes, me.L.bytes);
-      return -1;
-    }
-  }
+int split_run(Side* sd) {
+  for (int d = 0; d < 2; ++d) RC(side_layout(sd[d], d));
   if (sd[0].dev != sd[1].dev) {
     RC(enable_peer_access(sd[0].dev, sd[1].dev));
     RC(enable_peer_access(sd[1].dev, sd[0].dev));
   }
   for (int d = 0; d < 2; ++d) {
-    SplitSide& me = sd[d];
+    Side& me = sd[d];
     RC(check_cuda(cudaSetDevice(me.dev), "cudaSetDevice"));
     RC(check_cuda(cudaEventCreateWithFlags(&me.ready, cudaEventDisableTiming), "event create"));
     RC(check_cuda(cudaEventCreateWithFlags(&me.pulled, cudaEventDisableTiming), "event create"));
-    RC(run_prologue(me.e, me.L, me.sa, me.s));
-    if (sa->use_graph)
-      RC(step_graph(me.e, me.L, me.sa, me.ws, &me.g));
-    else
-      RC(build_step_plans(me.e, me.L, me.sa, me.P));
+    RC(side_prepare(me));
   }
-  return split_loop(sd, evals);
+  return split_loop(sd, sd[0].L.evals);
 }
 
 }  // namespace
@@ -1253,9 +1206,8 @@ extern "C" int f5_sample_cfg_split(f5_engine* e0, const f5_sample_args* a0, void
     return -1;
   }
   RC(check_problem("f5_sample_cfg_split", a0));
-  SplitSide sd[2];
-  sd[0].e = e0, sd[0].sa = a0, sd[0].ws = ws0, sd[0].bytes = ws0_bytes, sd[0].s = reinterpret_cast<cudaStream_t>(stream0);
-  sd[1].e = e1, sd[1].sa = a1, sd[1].ws = ws1, sd[1].bytes = ws1_bytes, sd[1].s = reinterpret_cast<cudaStream_t>(stream1);
+  Side sd[2] = {{e0, a0, ws0, ws0_bytes, reinterpret_cast<cudaStream_t>(stream0)},
+                {e1, a1, ws1, ws1_bytes, reinterpret_cast<cudaStream_t>(stream1)}};
   RC(split_check(sd));
   RC(pointer_device(ws0, "workspace 0", &sd[0].dev));
   RC(pointer_device(ws1, "workspace 1", &sd[1].dev));
@@ -1266,7 +1218,7 @@ extern "C" int f5_sample_cfg_split(f5_engine* e0, const f5_sample_args* a0, void
   // neither workspace is handed back while the other side may still read it.  Then the events go (destroying an event
   // with work pending is allowed: its resources are released once that work completes).
   for (int d = 0; d < 2; ++d) {
-    SplitSide &me = sd[d], &o = sd[1 - d];
+    Side &me = sd[d], &o = sd[1 - d];
     if (!me.ready || !o.pulled) continue;
     const cudaError_t err = cudaSetDevice(me.dev) != cudaSuccess ? cudaErrorInvalidDevice
                                                                   : cudaStreamWaitEvent(me.s, o.pulled, 0);

@@ -357,17 +357,8 @@ class _Backbone(nn.Module):
         stream = torch.cuda.current_stream(y.device).cuda_stream
         ws = self._ws_acquire(need, y.device, stream)
         tg = (C.c_float * (steps + 1))(*[float(v) for v in t_grid])
-        a = _lib.SampleArgs()
-        a.B, a.N, a.nt, a.steps = B, N, nt, steps
-        a.text, a.step_cond, a.y = text.data_ptr(), step_cond.data_ptr(), y.data_ptr()
-        a.duration = duration.data_ptr() if duration is not None else None
-        a.t = tg
-        a.cfg_strength = float(cfg_strength)
-        a.trajectory = trajectory.data_ptr() if trajectory is not None else None
-        a.use_graph = 1 if use_graph else 0
-        a.v_out = v_out.data_ptr() if v_out is not None else None
-        a.exact_varlen = 1 if (exact_varlen and duration is not None) else 0
-        a.method = _lib.ODE_METHODS[method]
+        a = _lib.sample_args(y, step_cond, text, duration, tg, steps, cfg_strength, trajectory, use_graph, exact_varlen,
+                             method, v_out)
         try:
             with torch.cuda.device(y.device):
                 _lib.check(L.f5_sample(st["handle"], C.byref(a), ws.data_ptr(), ws.numel(), stream), "f5_sample")

@@ -32,15 +32,14 @@ def _f(t: torch.Tensor) -> torch.Tensor:
 
 def packed_tensors(m) -> dict[str, torch.Tensor]:
     """Every operand the engine reads, in kernel layout, as a flat name -> tensor dict (the unit that is cached on disk).
-    Names: `time_w0`, `text_table`, `tb{i}.pw1_w`, `proj_w`, `conv_w{0,1}`, `L{i}.w_qkv`, `mod_w`, `out_w`, ..."""
+    Names: `time_w0`, `text_table`, `tb{i}.pw1_w`, `proj_w`, `conv_w{0,1}`, `L{i}.w_qkv`, `C{i}.w_qkv_c`, `mod_w`,
+    `out_w`, ..."""
     sd = {k: v for k, v in m.state_dict().items()}
     dev = next(m.parameters()).device
     if dev.type != "cuda":
         raise _lib.F5LibraryError("the backbone must live on a CUDA (H100) device before sampling; no CPU path exists")
     D, depth = m.dim, m.depth
-    if m.KIND == "MMDiT":
-        return _packed_mmdit(m, sd, dev)
-    dit = m.KIND == "DiT"
+    mmdit, unett = m.KIND == "MMDiT", m.KIND == "UNetT"
     T: dict[str, torch.Tensor] = {}
     T["time_w0"], T["time_b0"] = _h(sd["time_embed.time_mlp.0.weight"]), _f(sd["time_embed.time_mlp.0.bias"])
     T["time_w1"], T["time_b1"] = _h(sd["time_embed.time_mlp.2.weight"]), _f(sd["time_embed.time_mlp.2.bias"])
@@ -52,69 +51,40 @@ def packed_tensors(m) -> dict[str, torch.Tensor]:
         T[q + "pw1_w"], T[q + "pw1_b"] = _h(sd[p + "pwconv1.weight"]), _f(sd[p + "pwconv1.bias"])
         T[q + "grn_gamma"], T[q + "grn_beta"] = _f(sd[p + "grn.gamma"].reshape(-1)), _f(sd[p + "grn.beta"].reshape(-1))
         T[q + "pw2_w"], T[q + "pw2_b"] = _h(sd[p + "pwconv2.weight"]), _f(sd[p + "pwconv2.bias"])
-    pw = sd["input_embed.proj.weight"]
+    embed, proj = ("audio_embed.", "audio_embed.linear.") if mmdit else ("input_embed.", "input_embed.proj.")
+    pw = sd[proj + "weight"]
     kin = pw.shape[1]
     kpad = (kin + 63) // 64 * 64
     pwp = torch.zeros((D, kpad), dtype=torch.float16, device=dev)
     pwp[:, :kin] = pw.to(torch.float16)
-    T["proj_w"], T["proj_b"] = pwp, _f(sd["input_embed.proj.bias"])
+    T["proj_w"], T["proj_b"] = pwp, _f(sd[proj + "bias"])
     for j, idx in enumerate((0, 2)):
-        cw = sd[f"input_embed.conv_pos_embed.conv1d.{idx}.weight"]  # [D_out, G, 31]
-        T[f"conv_w{j}"] = _h(cw.permute(2, 0, 1))                     # [31, D_out, G]
-        T[f"conv_b{j}"] = _f(sd[f"input_embed.conv_pos_embed.conv1d.{idx}.bias"])
+        cw = sd[f"{embed}conv_pos_embed.conv1d.{idx}.weight"]  # [D_out, G, 31]
+        T[f"conv_w{j}"] = _h(cw.permute(2, 0, 1))              # [31, D_out, G]
+        T[f"conv_b{j}"] = _f(sd[f"{embed}conv_pos_embed.conv1d.{idx}.bias"])
+    mod = []  # AdaLN linears in table order (DiT, MMDiT)
     for i in range(depth):
         q = f"L{i}."
-        if dit:
-            p, a, f = f"transformer_blocks.{i}.", f"transformer_blocks.{i}.attn.", f"transformer_blocks.{i}.ff."
-        else:
+        if unett:
             p, a, f = f"layers.{i}.", f"layers.{i}.2.", f"layers.{i}.4."
+        else:
+            p, a = f"transformer_blocks.{i}.", f"transformer_blocks.{i}.attn."
+            f = p + ("ff_x." if mmdit else "ff.")
         T[q + "w_qkv"] = _h(torch.cat([sd[a + "to_q.weight"], sd[a + "to_k.weight"], sd[a + "to_v.weight"]], dim=0))
         T[q + "b_qkv"] = _f(torch.cat([sd[a + "to_q.bias"], sd[a + "to_k.bias"], sd[a + "to_v.bias"]], dim=0))
         T[q + "w_out"], T[q + "b_out"] = _h(sd[a + "to_out.0.weight"]), _f(sd[a + "to_out.0.bias"])
         T[q + "w_ff1"], T[q + "b_ff1"] = _h(sd[f + "ff.0.0.weight"]), _f(sd[f + "ff.0.0.bias"])
         T[q + "w_ff2"], T[q + "b_ff2"] = _h(sd[f + "ff.2.weight"]), _f(sd[f + "ff.2.bias"])
-        if not dit:
+        if unett:
             if (p + "0.weight") in sd:
                 T[q + "w_skip"] = _h(sd[p + "0.weight"])
             T[q + "g_attn"], T[q + "g_ff"] = _f(sd[p + "1.g"]), _f(sd[p + "3.g"])
         if m.qk_norm is not None:
             T[q + "q_norm_w"], T[q + "k_norm_w"] = _f(sd[a + "q_norm.weight"]), _f(sd[a + "k_norm.weight"])
-    if dit:
-        mw = [sd[f"transformer_blocks.{i}.attn_norm.linear.weight"] for i in range(depth)] + [sd["norm_out.linear.weight"]]
-        mb = [sd[f"transformer_blocks.{i}.attn_norm.linear.bias"] for i in range(depth)] + [sd["norm_out.linear.bias"]]
-        T["mod_w"], T["mod_b"] = _h(torch.cat(mw, dim=0)), _f(torch.cat(mb, dim=0))
-    else:
-        T["g_out"] = _f(sd["norm_out.g"])
-    T["out_w"], T["out_b"] = _h(sd["proj_out.weight"]), _f(sd["proj_out.bias"])
-    if m.long_skip:
-        T["long_skip_w"] = _h(sd["long_skip_connection.weight"])
-    return T
-
-
-def _packed_mmdit(m, sd, dev) -> dict[str, torch.Tensor]:
-    D, depth = m.dim, m.depth
-    T: dict[str, torch.Tensor] = {}
-    T["time_w0"], T["time_b0"] = _h(sd["time_embed.time_mlp.0.weight"]), _f(sd["time_embed.time_mlp.0.bias"])
-    T["time_w1"], T["time_b1"] = _h(sd["time_embed.time_mlp.2.weight"]), _f(sd["time_embed.time_mlp.2.bias"])
-    T["text_table"] = _f(sd["text_embed.text_embed.weight"])
-    pw = sd["audio_embed.linear.weight"]
-    kin = pw.shape[1]
-    kpad = (kin + 63) // 64 * 64
-    pwp = torch.zeros((D, kpad), dtype=torch.float16, device=dev)
-    pwp[:, :kin] = pw.to(torch.float16)
-    T["proj_w"], T["proj_b"] = pwp, _f(sd["audio_embed.linear.bias"])
-    for j, idx in enumerate((0, 2)):
-        cw = sd[f"audio_embed.conv_pos_embed.conv1d.{idx}.weight"]
-        T[f"conv_w{j}"] = _h(cw.permute(2, 0, 1))
-        T[f"conv_b{j}"] = _f(sd[f"audio_embed.conv_pos_embed.conv1d.{idx}.bias"])
-    mw, mb = [], []
-    for i in range(depth):
-        p, a, q, c = f"transformer_blocks.{i}.", f"transformer_blocks.{i}.attn.", f"L{i}.", f"C{i}."
-        T[q + "w_qkv"] = _h(torch.cat([sd[a + "to_q.weight"], sd[a + "to_k.weight"], sd[a + "to_v.weight"]], dim=0))
-        T[q + "b_qkv"] = _f(torch.cat([sd[a + "to_q.bias"], sd[a + "to_k.bias"], sd[a + "to_v.bias"]], dim=0))
-        T[q + "w_out"], T[q + "b_out"] = _h(sd[a + "to_out.0.weight"]), _f(sd[a + "to_out.0.bias"])
-        T[q + "w_ff1"], T[q + "b_ff1"] = _h(sd[p + "ff_x.ff.0.0.weight"]), _f(sd[p + "ff_x.ff.0.0.bias"])
-        T[q + "w_ff2"], T[q + "b_ff2"] = _h(sd[p + "ff_x.ff.2.weight"]), _f(sd[p + "ff_x.ff.2.bias"])
+        if not mmdit:
+            mod.append(p + "attn_norm.linear.")
+            continue
+        c = f"C{i}."  # the text stream; the last block has only its QKV (context_pre_only)
         T[c + "w_qkv_c"] = _h(torch.cat([sd[a + "to_q_c.weight"], sd[a + "to_k_c.weight"], sd[a + "to_v_c.weight"]], 0))
         T[c + "b_qkv_c"] = _f(torch.cat([sd[a + "to_q_c.bias"], sd[a + "to_k_c.bias"], sd[a + "to_v_c.bias"]], 0))
         if i < depth - 1:
@@ -122,14 +92,17 @@ def _packed_mmdit(m, sd, dev) -> dict[str, torch.Tensor]:
             T[c + "w_ff1_c"], T[c + "b_ff1_c"] = _h(sd[p + "ff_c.ff.0.0.weight"]), _f(sd[p + "ff_c.ff.0.0.bias"])
             T[c + "w_ff2_c"], T[c + "b_ff2_c"] = _h(sd[p + "ff_c.ff.2.weight"]), _f(sd[p + "ff_c.ff.2.bias"])
         if m.qk_norm is not None:
-            T[q + "q_norm_w"], T[q + "k_norm_w"] = _f(sd[a + "q_norm.weight"]), _f(sd[a + "k_norm.weight"])
             T[c + "q_norm_c"], T[c + "k_norm_c"] = _f(sd[a + "c_q_norm.weight"]), _f(sd[a + "c_k_norm.weight"])
-        mw += [sd[p + "attn_norm_x.linear.weight"], sd[p + "attn_norm_c.linear.weight"]]
-        mb += [sd[p + "attn_norm_x.linear.bias"], sd[p + "attn_norm_c.linear.bias"]]
-    mw.append(sd["norm_out.linear.weight"])
-    mb.append(sd["norm_out.linear.bias"])
-    T["mod_w"], T["mod_b"] = _h(torch.cat(mw, dim=0)), _f(torch.cat(mb, dim=0))
+        mod += [p + "attn_norm_x.linear.", p + "attn_norm_c.linear."]
+    if unett:
+        T["g_out"] = _f(sd["norm_out.g"])
+    else:
+        mod.append("norm_out.linear.")
+        T["mod_w"] = _h(torch.cat([sd[k + "weight"] for k in mod], dim=0))
+        T["mod_b"] = _f(torch.cat([sd[k + "bias"] for k in mod], dim=0))
     T["out_w"], T["out_b"] = _h(sd["proj_out.weight"]), _f(sd["proj_out.bias"])
+    if m.long_skip:
+        T["long_skip_w"] = _h(sd["long_skip_connection.weight"])
     return T
 
 

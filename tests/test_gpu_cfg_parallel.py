@@ -311,9 +311,9 @@ def split_abi(model, args, kw, peer):
     torch.cuda.synchronize(DEV)
     torch.cuda.synchronize(peer)
     tg = (C.c_float * 9)(*t)
-    a0 = cfg_parallel._args(y_a, sc, text, dur, tg, 8, 2.0, traj_a, True, False, "euler")
-    a1 = cfg_parallel._args(y1, sc.to(peer), text.to(peer), None if dur is None else dur.to(peer), tg, 8, 2.0, None,
-                            True, False, "euler")
+    a0 = _lib.sample_args(y_a, sc, text, dur, tg, 8, 2.0, traj_a, True, False, "euler")
+    a1 = _lib.sample_args(y1, sc.to(peer), text.to(peer), None if dur is None else dur.to(peer), tg, 8, 2.0, None,
+                          True, False, "euler")
     torch.cuda.synchronize(peer)
     _lib.check(L.f5_sample_cfg_split(st0["handle"], C.byref(a0), ws0.data_ptr(), need, s0.cuda_stream, st1["handle"],
                                      C.byref(a1), ws1.data_ptr(), need, s1.cuda_stream), "f5_sample_cfg_split")
@@ -353,8 +353,8 @@ def test_abi_rejects_mismatched_sides():
         return L.f5_sample_cfg_split(st["handle"], C.byref(a0), ws0.data_ptr(), need, s0.cuda_stream, st["handle"],
                                      C.byref(a1), ws1.data_ptr(), need, st1.cuda_stream)
 
-    args = lambda yy, steps=2, cfg_s=2.0: cfg_parallel._args(yy, sc, text, None, tg, steps, cfg_s, None, True,  # noqa
-                                                             False, "euler")
+    args = lambda yy, steps=2, cfg_s=2.0: _lib.sample_args(yy, sc, text, None, tg, steps, cfg_s, None, True,  # noqa
+                                                           False, "euler")
     assert call(args(y), args(y1, cfg_s=0.0)) != 0  # the two sides disagree
     assert call(args(y, cfg_s=0.0), args(y1, cfg_s=0.0)) != 0  # no unconditional half
     assert call(args(y), args(y)) != 0  # one y for both sides
