@@ -49,7 +49,8 @@ def seed_everything(seed=0):
 
 class F5TTS:
     def __init__(self, model="F5TTS_v1_Base", ckpt_file="", vocab_file="", ode_method="euler", use_ema=True,
-                 vocoder_local_path=None, device=None, hf_cache_dir=None, cfg_parallel_device=None):
+                 vocoder_local_path=None, device=None, hf_cache_dir=None, cfg_parallel_device=None,
+                 sample_parallel_devices=None):
         if model not in MODEL_ARCH:
             raise ValueError(f"unknown model {model!r}; shipped configs: {sorted(MODEL_ARCH)}")
         model_cls, model_arc = MODEL_ARCH[model]
@@ -64,7 +65,8 @@ class F5TTS:
                                     "(api.py:65-81 in the reference downloads it)")
         self.ema_model = _infer.load_model(model_cls, model_arc, ckpt_file, self.mel_spec_type, vocab_file,
                                            self.ode_method, self.use_ema, self.device,
-                                           cfg_parallel_device=cfg_parallel_device)
+                                           cfg_parallel_device=cfg_parallel_device,
+                                           sample_parallel_devices=sample_parallel_devices)
         self.seed = None
 
     def export_wav(self, wav, file_wave, remove_silence=False):

@@ -12,6 +12,8 @@ The peer holds a replica of the backbone's packed operands, copied again wheneve
 changes, its own stream and its own workspace pool.  The peer may be the model's own device ("loopback": two workspaces
 on one GPU, the same engine); that runs the same code path and is how one GPU tests it.  Whether the pair is faster than
 one GPU depends on the size of the call (DESIGN.md §8), which is why it is off by default.
+
+`DevicePeer` is that per-device state on its own; the sample split (`sample_parallel.py`) runs its groups on it too.
 """
 from __future__ import annotations
 
@@ -23,18 +25,19 @@ import torch
 from . import _lib
 
 
-def peer_device(device) -> torch.device:
-    """The CUDA device `device` names; ValueError for a CPU or unknown device."""
+def peer_device(device, what: str = "cfg_parallel device") -> torch.device:
+    """The CUDA device `device` names; ValueError for a CPU or unknown device.  `what` names the argument in the
+    message."""
     try:
         dev = torch.device(device)
     except (RuntimeError, TypeError) as e:
-        raise ValueError(f"cfg_parallel device {device!r}: {e}") from None
+        raise ValueError(f"{what} {device!r}: {e}") from None
     if dev.type != "cuda":
-        raise ValueError(f"cfg_parallel device {device!r} is not a CUDA device: the peer half runs on a GPU")
+        raise ValueError(f"{what} {device!r} is not a CUDA device: split calls run on a GPU")
     count = torch.cuda.device_count() if torch.cuda.is_available() else 0
     index = dev.index if dev.index is not None else (torch.cuda.current_device() if count else 0)
     if index >= count:
-        raise ValueError(f"cfg_parallel device {device!r}: this process sees {count} CUDA device(s)")
+        raise ValueError(f"{what} {device!r}: this process sees {count} CUDA device(s)")
     return torch.device("cuda", index)
 
 
@@ -56,8 +59,8 @@ def destroy(state: dict) -> None:
     _lib.lib().f5_engine_destroy(state["handle"])
 
 
-class CfgPeer:
-    """The peer side of split calls for one backbone: the device, the replica engine, a stream, a workspace pool.
+class DevicePeer:
+    """One device's side of split calls for one backbone: the device, the replica engine, a stream, a workspace pool.
 
     `copy_weights`: None (default) replicates the weights when the peer is another device and runs loopback on the
     primary's own engine; True replicates them even on the primary's device (two engines on one GPU, which exercises
@@ -74,7 +77,7 @@ class CfgPeer:
         self.replications = 0  # replicas made so far (one per primary fingerprint the peer has served)
 
     def engine(self, backbone, primary: dict, primary_device: torch.device) -> dict:
-        """The engine the peer half runs on: the primary's own for loopback, else the replica, copied again when the
+        """The engine the peer's work runs on: the primary's own for loopback, else the replica, copied again when the
         primary's fingerprint (the `fp` its engine state was packed at) has changed."""
         if primary_device == self.device and not self.copy_weights:
             return primary
@@ -120,6 +123,10 @@ class CfgPeer:
                 destroy(st)
             except Exception:
                 pass
+
+
+class CfgPeer(DevicePeer):
+    """The peer side of CFG-split calls: a `DevicePeer` that runs the unconditional half."""
 
     def run(self, backbone, y, step_cond, text, t_grid, duration, cfg_strength, trajectory, use_graph, exact_varlen,
             method):

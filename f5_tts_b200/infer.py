@@ -196,12 +196,14 @@ def load_checkpoint(model, ckpt_path, device: str, dtype=None, use_ema=True):
 
 
 def load_model(model_cls, model_cfg, ckpt_path, mel_spec_type=mel_spec_type, vocab_file="", ode_method=ode_method,
-               use_ema=True, device=device, packed_cache_dir=None, cfg_parallel_device=None):
+               use_ema=True, device=device, packed_cache_dir=None, cfg_parallel_device=None,
+               sample_parallel_devices=None):
     """utils_infer.py:238-276.  `packed_cache_dir` (extra, default off): keep the kernel-layout operands of this
     checkpoint (fp16 K-major weights, stacked QKV / AdaLN matrices, re-tiled conv weights; weights.py) in that folder and
     read them straight onto the GPU on later loads instead of re-packing 0.67 GB through conversion kernels.
     `cfg_parallel_device` (extra, default off): run the unconditional CFG half of every sampler call on that GPU
-    (CFM.enable_cfg_parallel)."""
+    (CFM.enable_cfg_parallel).  `sample_parallel_devices` (extra, default off): run the samples of every batched sampler
+    call in groups on those GPUs (CFM.enable_sample_parallel)."""
     if vocab_file == "":
         raise FileNotFoundError("vocab_file is required (the reference defaults to its packaged "
                                 "infer/examples/vocab.txt, utils_infer.py:248-249; that data file is not vendored here)")
@@ -224,6 +226,8 @@ def load_model(model_cls, model_cfg, ckpt_path, mel_spec_type=mel_spec_type, voc
                 _w.save_packed(model.transformer, path)
     if cfg_parallel_device is not None:
         model.enable_cfg_parallel(cfg_parallel_device)
+    if sample_parallel_devices is not None:
+        model.enable_sample_parallel(sample_parallel_devices)
     return model
 
 

@@ -25,7 +25,7 @@ import torch.nn.functional as F
 from torch import nn
 from torch.nn.utils.rnn import pad_sequence
 
-from . import _lib, batching, cfg_parallel
+from . import _lib, batching, cfg_parallel, sample_parallel
 
 # ----------------------------------------------------------------------------------------------------------------
 # small host helpers (model/utils.py)
@@ -274,6 +274,7 @@ class _Backbone(nn.Module):
         self._ws_lock = threading.Lock()
         self._ws_free: dict = {}  # (device, stream) -> [uint8 tensors] not in use by a sample() call
         self.cfg_peer = None  # a cfg_parallel.CfgPeer while CFM.enable_cfg_parallel() is on
+        self.sample_split = None  # a sample_parallel.SampleSplit while CFM.enable_sample_parallel() is on
 
     # -- engine management ------------------------------------------------------------------------------------
     def _fingerprint(self):
@@ -336,7 +337,12 @@ class _Backbone(nn.Module):
         """One engine call = len(t_grid)-1 steps of the fixed-grid ODE `method` ("euler": one backbone evaluation per
         step, "midpoint": two).  All tensors on the CUDA device, fp32 / int64 / int32.  With a CFG peer set
         (CFM.enable_cfg_parallel) a call with guidance runs its unconditional half there; one without (cfg_strength
-        < 1e-5) or one that asks for the raw backbone output (v_out) runs here alone."""
+        < 1e-5) or one that asks for the raw backbone output (v_out) runs here alone.  With a sample split set
+        (CFM.enable_sample_parallel) a call of two or more samples without v_out runs its samples in groups there."""
+        split = self.sample_split
+        if split is not None and v_out is None and y.shape[0] >= 2:
+            return split.run(self, y, step_cond, text, t_grid, duration, cfg_strength, trajectory, use_graph,
+                             exact_varlen, method)
         peer = self.cfg_peer
         if peer is not None and v_out is None and float(cfg_strength) >= 1e-5:
             return peer.run(self, y, step_cond, text, t_grid, duration, cfg_strength, trajectory, use_graph,
@@ -529,7 +535,10 @@ class CFM(nn.Module):
         the model's own device (two workspaces on one GPU).  Calls with cfg_strength < 1e-5 and the backbone's
         `forward` stay on the model's device.  Merged runs of `enable_batching` split too.  ValueError for a CPU or
         unknown device.  Enabling it again for the same device keeps the peer (its weight copy, stream, workspaces and
-        captured graphs).  Returns the peer."""
+        captured graphs).  ValueError while the sample split (`enable_sample_parallel`) is on.  Returns the peer."""
+        if self.transformer.sample_split is not None:
+            raise ValueError("the sample split is on: disable_sample_parallel() first (the CFG split and the sample "
+                             "split do not run together)")
         dev = cfg_parallel.peer_device(device)
         peer = self.transformer.cfg_peer
         if peer is None or peer.device != dev:
@@ -541,6 +550,34 @@ class CFM(nn.Module):
         """Later `sample()` calls run on the model's device alone again; the peer's weight copy and workspaces go once
         no call uses them."""
         self.transformer.cfg_peer = None
+
+    def enable_sample_parallel(self, devices) -> list[cfg_parallel.DevicePeer]:
+        """Run the samples of every `sample()` call of B >= 2 samples in groups, one group per entry of `devices`
+        (f5_tts_b200/sample_parallel.py).
+
+        The batch is cut into at most len(devices) contiguous groups that balance the work; each group is an ordinary
+        engine call on its device, with no exchange during the ODE loop, so every call returns what it returns without
+        this, bit for bit on every frame the call's mode defines (with `exact_varlen=True` the trajectory's frames past
+        a sample's duration are zero).  Each device holds a replica of
+        the backbone's packed weights, copied again when the weights change; a device may be the model's own and may
+        be named more than once (more streams and workspaces on one GPU).  Calls of one sample and the backbone's
+        `forward` stay on the model's device; merged runs of `enable_batching` split too.  ValueError for an empty list,
+        a CPU or unknown device, or while the CFG split (`enable_cfg_parallel`) is on.  Enabling it again with the same
+        list keeps the peers (weight copies, streams, workspaces and captured graphs).  Returns the peers, in order."""
+        if self.transformer.cfg_peer is not None:
+            raise ValueError("the CFG split is on: disable_cfg_parallel() first (the CFG split and the sample split do "
+                             "not run together)")
+        devs = sample_parallel.split_devices(devices)
+        split = self.transformer.sample_split
+        if split is None or [p.device for p in split.peers] != devs:
+            split = sample_parallel.SampleSplit(devs)
+            self.transformer.sample_split = split
+        return split.peers
+
+    def disable_sample_parallel(self) -> None:
+        """Later `sample()` calls run on the model's device alone again; the peers' weight copies and workspaces go
+        once no call uses them."""
+        self.transformer.sample_split = None
 
     @property
     def device(self):
