@@ -83,6 +83,17 @@ class SampleArgs(C.Structure):
     ]
 
 
+class ForwardArgs(C.Structure):  # f5_forward_args: one backbone evaluation (the reference's transformer operator)
+    _fields_ = [
+        ("B", c_int), ("N", c_int), ("nt", c_int),
+        ("x", c_void_p), ("step_cond", c_void_p), ("text", c_void_p), ("duration", c_void_p), ("time", c_void_p),
+        ("mode", c_int), ("v_out", c_void_p), ("use_graph", c_int), ("reuse_text", c_int),
+    ]
+
+
+# ForwardArgs.mode: the conditional flow, cond | uncond packed (cfg_infer), the unconditional flow (joint drop)
+FORWARD_COND, FORWARD_CFG, FORWARD_UNCOND = 0, 1, 2
+
 ODE_METHODS = {"euler": 0, "midpoint": 1}
 BACKBONES = {"DiT": 0, "UNetT": 1, "MMDiT": 2}  # Arch.backbone  # SampleArgs.method; backbone evaluations per grid interval: 1 and 2
 SKIP_TYPES = {"concat": 0, "add": 1, "none": 2}  # Arch.skip_type: UNetT skip_connect_type
@@ -161,9 +172,14 @@ def lib():
                                           c_void_p, C.POINTER(SampleArgs), c_void_p, c_size_t, c_void_p]
         L.f5_sample_cfg_split_workspace_bytes.argtypes = [c_void_p, c_int, c_int, c_int, c_int]
         L.f5_sample_cfg_split_workspace_bytes.restype = c_size_t
+        L.f5_forward.argtypes = [c_void_p, C.POINTER(ForwardArgs), c_void_p, c_size_t, c_void_p]
+        L.f5_forward_workspace_bytes.argtypes = [c_void_p, c_int, c_int, c_int, c_int]
+        L.f5_forward_workspace_bytes.restype = c_size_t
+        L.f5_engine_graph_count.argtypes = [c_void_p]
+        L.f5_engine_graph_count.restype = c_int
         for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_attention_joint", "f5_row_norm", "f5_mel_spectrogram",
                      "f5_vocos_decode",
-                     "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample", "f5_sample_cfg_split"):
+                     "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample", "f5_sample_cfg_split", "f5_forward"):
             getattr(L, name).restype = c_int
         _lib = L
     return _lib
@@ -184,7 +200,8 @@ EXPORTED_SYMBOLS = [
     "f5_row_norm", "f5_mel_spectrogram",
     "f5_vocos_workspace_bytes", "f5_vocos_decode", "f5_vocos_decode_varlen", "f5_engine_create", "f5_engine_destroy",
     "f5_sample_workspace_bytes", "f5_sample", "f5_sample_flops", "f5_attention_joint", "f5_sample_workspace_bytes_nt",
-    "f5_sample_flops_nt", "f5_sample_cfg_split", "f5_sample_cfg_split_workspace_bytes",
+    "f5_sample_flops_nt", "f5_sample_cfg_split", "f5_sample_cfg_split_workspace_bytes", "f5_forward",
+    "f5_forward_workspace_bytes", "f5_engine_graph_count",
 ]
 
 # Test-only library: the same objects plus one extern "C" wrapper per kernel launcher (csrc/kernel_hooks.cu), used by
@@ -194,5 +211,5 @@ KERNEL_HOOK_SYMBOLS = [
     "f5k_last_error", "f5k_row_norm", "f5k_dwconv7_ln", "f5k_text_gather", "f5k_mask_rows", "f5k_mask_rows_len",
     "f5k_grn_rows", "f5k_grn", "f5k_pack_input", "f5k_cfg_euler", "f5k_small_linear", "f5k_time_features",
     "f5k_silu_to_half", "f5k_rope_table", "f5k_prepend_time_token", "f5k_concat_half", "f5k_vocos_im2col",
-    "f5k_ln_affine_f32", "f5k_istft", "f5k_row_norm_add_skip",
+    "f5k_ln_affine_f32", "f5k_istft", "f5k_row_norm_add_skip", "f5k_gemm_resid_sample",
 ]

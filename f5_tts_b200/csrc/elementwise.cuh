@@ -14,12 +14,14 @@ namespace f5 {
 //   MODE 2: x / max(||x||, 1e-12) * sqrt(D) * g[c]                     (x_transformers RMSNorm, unett.py:154)
 //   MODE 3: x += skip (fp32, written back to x), then MODE 2 of the sum (UNetT skip_connect_type="add": the
 //           `x = x + skip` that opens each later-half layer fused into its attn_norm, unett.py:296-297)
-// scale/shift live in the per-step modulation table: ptr + (*step_ptr) * step_stride.
+//   MODE 4: MODE 0 with the modulation row of each row's sample (f5_forward: one time per sample)
+// scale/shift live in the per-step modulation table: ptr + (*step_ptr) * step_stride; MODE 4 reads
+// ptr + ((row / sample_seq) % samples) * step_stride.
 // ---------------------------------------------------------------------------------------------------------
 
 template <int MODE>
 __global__ void __launch_bounds__(256) row_norm_kernel(const NormParams p) {
-  constexpr bool kAffine = MODE == 0 || MODE == 1;  // LayerNorm with a second parameter row (shift / bias)
+  constexpr bool kAffine = MODE == 0 || MODE == 1 || MODE == 4;  // LayerNorm with a second parameter row (shift / bias)
   pdl_launch_dependents();
   const int row = blockIdx.x * int(blockDim.x >> 5) + (threadIdx.x >> 5);  // one warp per row
   const int lane = lane_id();
@@ -30,7 +32,9 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const NormParams p) {
   // step counter of the previous NFE step), so they are fetched BEFORE the programmatic-launch dependency wait — the
   // block is already resident while the residual GEMM is still running, and only the x rows are left to read after it.
   auto load_params = [&]() {
-    const long long so = p.step_ptr ? (long long)(*p.step_ptr) * p.step_stride : 0;
+    const long long so = MODE == 4   ? (long long)((row / p.sample_seq) % p.samples) * p.step_stride
+                         : p.step_ptr ? (long long)(*p.step_ptr) * p.step_stride
+                                      : 0;
     const float4* A = reinterpret_cast<const float4*>(p.a + so);
     const float4* B = kAffine ? reinterpret_cast<const float4*>(p.b + so) : nullptr;
 #pragma unroll
@@ -96,7 +100,7 @@ __global__ void __launch_bounds__(256) row_norm_kernel(const NormParams p) {
     if (i < nv) {
       const float4 a = ga[i];
       float4 r;
-      if (MODE == 0) {
+      if (MODE == 0 || MODE == 4) {
         const float4 b = gb[i];
         r.x = (v[i].x - mean) * rstd * (1.f + a.x) + b.x;
         r.y = (v[i].y - mean) * rstd * (1.f + a.y) + b.y;
@@ -497,6 +501,19 @@ __global__ void prepend_time_token_kernel(float* dst, const float* src, const fl
   const long long b = row / (N + 1);
   const int n = int(row % (N + 1));
   const float* s = (n == 0) ? t_emb + (long long)(*step_ptr) * D : src + (b * N + (n - 1)) * D;
+  for (int c = threadIdx.x; c < D; c += blockDim.x) dst[row * D + c] = s[c];
+}
+
+// f5_forward: the same with each sample's own time embedding, t_emb[b % samples] (cond and uncond rows share it)
+__global__ void prepend_time_token_sample_kernel(float* dst, const float* src, const float* t_emb, int samples, int N,
+                                                 int D, long long rows_out) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const long long row = blockIdx.x;
+  if (row >= rows_out) return;
+  const long long b = row / (N + 1);
+  const int n = int(row % (N + 1));
+  const float* s = (n == 0) ? t_emb + (b % samples) * D : src + (b * N + (n - 1)) * D;
   for (int c = threadIdx.x; c < D; c += blockDim.x) dst[row * D + c] = s[c];
 }
 

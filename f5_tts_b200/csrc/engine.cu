@@ -64,6 +64,9 @@ struct Layout {
   // computes only the conditional / unconditional half: Be = B rows of work, while xin, v and the MMDiT text embedding
   // keep both halves (Bx = 2B samples) so that the unchanged update kernel runs over the full v
   int half, Bx;
+  // f5_forward: the time and modulation tables hold one row per sample (evals = B), and every reader takes the row of
+  // its sample (b % B: the cond and uncond rows of a sample share it) instead of the evaluation counter's
+  bool per_sample;
   long long M;  // Be * N mel frames (the audio stream's rows without the UNetT time token)
   // common
   int* step_ptr;    // [0]: evaluation counter
@@ -131,14 +134,24 @@ struct GraphKey {
            // depend on it (keying them on it would re-capture whenever text lengths differ)
   int half;  // Layout::half: -1 for f5_sample's graph (the whole evaluation), 0 / 1 for one CFG half of a split call
              // (the evaluation up to proj_out: the exchange and the update run outside the graph)
+  int forward;  // 1: an f5_forward graph (one evaluation up to proj_out with per-sample modulation rows)
   bool operator==(const GraphKey& o) const {
     return ws == o.ws && B == o.B && N == o.N && evals == o.evals && packed == o.packed && masked == o.masked &&
-           nt == o.nt && half == o.half;
+           nt == o.nt && half == o.half && forward == o.forward;
   }
 };
 struct GraphEntry {
   GraphKey key;
   std::shared_ptr<GraphHolder> g;
+};
+
+// The problem whose text embeddings an f5_forward call left in a workspace (f5_forward_args.reuse_text checks it)
+struct TextHeld {
+  const void* ws;
+  int B, N, nt, mode, masked;
+  bool operator==(const TextHeld& o) const {
+    return ws == o.ws && B == o.B && N == o.N && nt == o.nt && mode == o.mode && masked == o.masked;
+  }
 };
 
 struct f5_engine {
@@ -149,6 +162,7 @@ struct f5_engine {
   int inner, modW, kin;
   std::mutex mu;
   std::vector<GraphEntry> graphs;
+  std::vector<TextHeld> text_held;  // under mu
 };
 
 static constexpr int kDiT = 0, kUNetT = 1, kMMDiT = 2;  // f5_arch.backbone
@@ -173,6 +187,7 @@ static void plan_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, i
   L.N = N;
   L.evals = evals;
   L.half = half;
+  L.per_sample = false;
   L.packed = (cfg < 1e-5f && half < 0) ? 0 : 1;
   L.Be = (L.packed && half < 0) ? 2 * B : B;
   L.Bx = L.packed ? 2 * B : B;
@@ -468,6 +483,15 @@ f5_gemm_args base_args(long long rows, int n_out, int k, int lda, int ldw, int b
 
 constexpr int kAutoTile = 0;  // bn = 0: the GEMM planner picks the tile shape per problem (gemm.cu: pick_tile)
 
+// f5_forward: a gated residual GEMM reads the AdaLN gate row of each output row's sample (EPI_RESID_SAMPLE).  The tile
+// width stays the one the planner picked for EPI_RESID, so each output element is computed exactly as in f5_sample.
+void gate_per_sample(const Layout& L, const TokenStream& st, GemmPlan& pl) {
+  if (!L.per_sample || pl.p.gate == nullptr) return;
+  pl.epi = EPI_RESID_SAMPLE;
+  pl.p.gate_seq = st.seq;
+  pl.p.gate_samples = L.B;
+}
+
 // The four GEMMs of one block of one stream: QKV (+ per-head RMSNorm) + RoPE on the first pe_heads heads, out-projection
 // (+ gate, + zeroed padded rows, + residual), FF1 + GELU, FF2 (+ gate, + residual).  m: the block's AdaLN vectors of
 // this stream (gates at 2D and 5D), or null (UNetT: no gates).  qkv_only: MMDiT's last text block (context_pre_only).
@@ -517,6 +541,7 @@ int plan_block(const f5_engine* e, const Layout& L, const TokenStream& st, const
     gate(a, 2);
     varlen(a);
     RC(gemm_plan(&P.oproj, st.ao, lw.w_out, &a));
+    gate_per_sample(L, st, P.oproj);
   }
   {
     f5_gemm_args a = base_args(st.rows, F, D, D, D, kAutoTile, F5_EPI_F16, F5_ACT_GELU_TANH);
@@ -534,6 +559,7 @@ int plan_block(const f5_engine* e, const Layout& L, const TokenStream& st, const
     gate(a, 5);
     varlen(a);
     RC(gemm_plan(&P.ff2, st.g, lw.w_ff2, &a));
+    gate_per_sample(L, st, P.ff2);
   }
   return 0;
 }
@@ -664,8 +690,13 @@ int norm_mod(const f5_engine* e, const Layout& L, const TokenStream& st, int mod
   p.eps = 1e-6f;
   p.a = a;
   p.b = b;
-  p.step_ptr = step_indexed ? L.step_ptr : nullptr;
+  p.step_ptr = step_indexed && !L.per_sample ? L.step_ptr : nullptr;
   p.step_stride = step_indexed ? e->modW : 0;
+  if (step_indexed && L.per_sample) {  // AdaLN (mode 0) with the row of each row's sample
+    mode = 4;
+    p.sample_seq = st.seq;
+    p.samples = L.B;
+  }
   p.params_static = 1;  // modulation table / gains: complete long before the GEMM that produces x
   if (diag_skip("norm")) return 0;
   return run_row_norm(mode, p, s);
@@ -732,7 +763,9 @@ int run_body(f5_engine* e, const Layout& L, const StepPlans& P, cudaStream_t s) 
     RC(gemm_run(P.conv1, s));
     RC(gemm_run(P.conv2, s));
   }
-  if (A.backbone == kUNetT) RC(run_prepend_time_token(L.x.res, L.h0, L.temb, L.step_ptr, L.N, D, L.x.rows, s));
+  if (A.backbone == kUNetT)
+    RC(L.per_sample ? run_prepend_time_token_per_sample(L.x.res, L.h0, L.temb, L.B, L.N, D, L.x.rows, s)
+                    : run_prepend_time_token(L.x.res, L.h0, L.temb, L.step_ptr, L.N, D, L.x.rows, s));
   if (A.backbone == kMMDiT) {
     // the text stream restarts from its embedding at every evaluation (get_input_embed, mmdit.py:177-196)
     RC(check_cuda(cudaMemcpyAsync(L.c.res, L.c0, sizeof(float) * L.c.rows * D, cudaMemcpyDeviceToDevice, s),
@@ -780,68 +813,43 @@ int run_step(f5_engine* e, const Layout& L, const StepPlans& P, cudaStream_t s) 
   return run_update(e, L, s);
 }
 
-int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaStream_t s) {
+// Per-sample lengths of a call with durations (device int32 [B]): row, key, frame and valid lengths, and the buffer clears
+// that tile skipping relies on
+int set_lengths(f5_engine* e, const Layout& L, const int* duration, bool exact_varlen, cudaStream_t s) {
+  const f5_arch& A = e->arch;
+  const int D = A.dim, B = L.B;
+  // row_len[Be] = duration (+1 for the UNetT time token, unett.py:274-275); kv_len likewise
+  std::vector<int> hd(B);
+  RC(check_cuda(cudaMemcpyAsync(hd.data(), duration, sizeof(int) * B, cudaMemcpyDeviceToHost, s), "dur d2h"));
+  RC(check_cuda(cudaStreamSynchronize(s), "dur sync"));
+  std::vector<int> rl(L.Be);
+  for (int i = 0; i < L.Be; ++i) rl[i] = hd[i % B] + (A.backbone == kUNetT ? 1 : 0);
+  RC(check_cuda(cudaMemcpyAsync(L.row_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "row_len"));
+  RC(check_cuda(cudaMemcpyAsync(L.kv_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "kv_len"));
+  RC(check_cuda(cudaMemcpyAsync(L.valid_len, hd.data(), sizeof(int) * B, cudaMemcpyHostToDevice, s), "valid_len"));
+  std::vector<int> fl(L.Be);
+  for (int i = 0; i < L.Be; ++i) fl[i] = hd[i % B];
+  RC(check_cuda(cudaMemcpyAsync(L.frame_len, fl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "frame_len"));
+  RC(check_cuda(cudaStreamSynchronize(s), "len sync"));
+  if (A.attn_mask_enabled || exact_varlen) {
+    // tile skipping leaves padded rows of these buffers unwritten for the whole call: the conv inputs must read as
+    // zero there (= the conv's padding), and q/k/v rows next to a sample's end are multiplied by P = 0 (must be finite)
+    RC(check_cuda(cudaMemsetAsync(L.h0h, 0, sizeof(__half) * L.M * D, s), "h0h clear"));
+    RC(check_cuda(cudaMemsetAsync(L.c1, 0, sizeof(__half) * L.M * D, s), "c1 clear"));
+    RC(check_cuda(cudaMemsetAsync(L.x.qkv, 0, sizeof(__half) * L.x.rows * 3 * e->inner, s), "qkv clear"));
+  }
+  return 0;
+}
+
+// Time embedding of the L.evals times in t_dev (modules.py:852-862) and, DiT / MMDiT, their rows of the AdaLN table
+int run_time_embed(f5_engine* e, const Layout& L, cudaStream_t s) {
   const f5_arch& A = e->arch;
   const f5_weights& W = e->w;
-  const int D = A.dim, Td = A.text_dim, B = L.B, N = L.N, S = L.evals;
-  const bool dit = A.backbone == kDiT;
-  const bool mmdit = A.backbone == kMMDiT;
-  const bool masked = sa->duration != nullptr;
-  const bool strict = masked && sa->exact_varlen;
-  // small host -> device control data (pageable source: cudaMemcpyAsync stages it before returning).
-  // Per grid interval k (torchdiffeq's fixed-grid solvers): Euler evaluates at t_k and commits y + dt_k * g; midpoint
-  // evaluates at t_k, forms y + half_dt_k * g as the next evaluation's input only, then evaluates at t_k + half_dt_k
-  // and commits y + dt_k * g.  Times are fp32 (the reference builds the grid in the parameter dtype).
-  std::vector<OdeStage> stage;
-  std::vector<float> te;
-  stage.reserve(S);
-  te.reserve(S);
-  for (int k = 0; k < sa->steps; ++k) {
-    const float dt = sa->t[k + 1] - sa->t[k];
-    if (sa->method == 1) {
-      const float half_dt = 0.5f * dt;
-      te.push_back(sa->t[k]);
-      stage.push_back(OdeStage{half_dt, -1});
-      te.push_back(sa->t[k] + half_dt);
-      stage.push_back(OdeStage{dt, k + 1});
-    } else {
-      te.push_back(sa->t[k]);
-      stage.push_back(OdeStage{dt, k + 1});
-    }
-  }
-  RC(check_cuda(cudaMemcpyAsync(L.stage, stage.data(), sizeof(OdeStage) * S, cudaMemcpyHostToDevice, s), "stage h2d"));
-  RC(check_cuda(cudaMemcpyAsync(L.t_dev, te.data(), sizeof(float) * S, cudaMemcpyHostToDevice, s), "t h2d"));
-  RC(check_cuda(cudaMemsetAsync(L.step_ptr, 0, sizeof(int) * 64, s), "step memset"));
-  SampleIo io{sa->y, sa->trajectory, sa->cfg_strength};
-  RC(check_cuda(cudaMemcpyAsync(L.io, &io, sizeof(io), cudaMemcpyHostToDevice, s), "io h2d"));
-  if (masked) {
-    // row_len[Be] = duration (+1 for the UNetT time token, unett.py:274-275); kv_len likewise
-    std::vector<int> hd(B);
-    RC(check_cuda(cudaMemcpyAsync(hd.data(), sa->duration, sizeof(int) * B, cudaMemcpyDeviceToHost, s), "dur d2h"));
-    RC(check_cuda(cudaStreamSynchronize(s), "dur sync"));
-    std::vector<int> rl(L.Be);
-    for (int i = 0; i < L.Be; ++i) rl[i] = hd[i % B] + (A.backbone == kUNetT ? 1 : 0);
-    RC(check_cuda(cudaMemcpyAsync(L.row_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "row_len"));
-    RC(check_cuda(cudaMemcpyAsync(L.kv_len, rl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "kv_len"));
-    RC(check_cuda(cudaMemcpyAsync(L.valid_len, hd.data(), sizeof(int) * B, cudaMemcpyHostToDevice, s), "valid_len"));
-    std::vector<int> fl(L.Be);
-    for (int i = 0; i < L.Be; ++i) fl[i] = hd[i % B];
-    RC(check_cuda(cudaMemcpyAsync(L.frame_len, fl.data(), sizeof(int) * L.Be, cudaMemcpyHostToDevice, s), "frame_len"));
-    RC(check_cuda(cudaStreamSynchronize(s), "len sync"));
-    if (A.attn_mask_enabled || sa->exact_varlen) {
-      // tile skipping leaves padded rows of these buffers unwritten for the whole call: the conv inputs must read as
-      // zero there (= the conv's padding), and q/k/v rows next to a sample's end are multiplied by P = 0 (must be finite)
-      RC(check_cuda(cudaMemsetAsync(L.h0h, 0, sizeof(__half) * L.M * D, s), "h0h clear"));
-      RC(check_cuda(cudaMemsetAsync(L.c1, 0, sizeof(__half) * L.M * D, s), "c1 clear"));
-      RC(check_cuda(cudaMemsetAsync(L.x.qkv, 0, sizeof(__half) * L.x.rows * 3 * e->inner, s), "qkv clear"));
-    }
-  }
-  RC(run_rope_table(L.x.rope_cos, L.x.rope_sin, L.x.seq, A.dim_head / 2, s));
-  // time embedding for every evaluation time (modules.py:852-862)
+  const int D = A.dim, S = L.evals;
   RC(run_time_features(L.t_dev, L.tfeat, S, 256, s));
   RC(run_small_linear(1, L.tfeat, reinterpret_cast<const __half*>(W.time_w0), W.time_b0, L.th1, S, 256, D, s));
   RC(run_small_linear(0, L.th1, reinterpret_cast<const __half*>(W.time_w1), W.time_b1, L.temb, S, D, D, s));
-  if (dit || mmdit) {
+  if (A.backbone == kDiT || A.backbone == kMMDiT) {
     RC(run_silu_to_half(L.temb, L.temb_silu, (long long)S * D, s));
     f5_gemm_args a = base_args(S, e->modW, D, D, D, 128, F5_EPI_F32, F5_ACT_NONE);
     a.bias = W.mod_b;
@@ -851,16 +859,27 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
     RC(gemm_plan(&pl, L.temb_silu, W.mod_w, &a));
     RC(gemm_run(pl, s));
   }
+  return 0;
+}
+
+// Text embedding of both CFG variants (dit.py:86-139 / unett.py:55-84; MMDiT: mmdit.py:42-60 and its rope table).
+// masked: durations were given (set_lengths wrote valid_len); strict: exact_varlen.
+int run_text_embed(f5_engine* e, const Layout& L, const long long* text, int nt, bool masked, bool strict,
+                   cudaStream_t s) {
+  const f5_arch& A = e->arch;
+  const f5_weights& W = e->w;
+  const int D = A.dim, Td = A.text_dim, B = L.B, N = L.N;
+  const bool dit = A.backbone == kDiT;
+  const bool mmdit = A.backbone == kMMDiT;
   if (mmdit) {  // text embedding of both CFG variants and the text rope table; no text columns in the input projection
-    RC(run_mmdit_text_embed(sa->text, B, L.Bx, L.c.seq, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding,
+    RC(run_mmdit_text_embed(text, B, L.Bx, L.c.seq, D, W.text_table, A.text_num_embeds + 1, A.text_mask_padding,
                             L.c0_all, L.c_len_all, s));
     RC(run_rope_table(L.c.rope_cos, L.c.rope_sin, L.c.seq, A.dim_head / 2, s));
   }
-  // text embedding, both CFG variants (dit.py:86-139 / unett.py:55-84)
   TextGatherParams tp{};
-  tp.ids = sa->text;
+  tp.ids = text;
   tp.B = B;
-  tp.nt = sa->nt;
+  tp.nt = nt;
   tp.N = N;
   tp.Td = Td;
   tp.valid_len = (dit && masked) ? L.valid_len : nullptr;
@@ -903,21 +922,65 @@ int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaSt
   }
   if (A.conv_layers > 0 && A.text_mask_padding) RC(run_mask_rows(L.tx, L.filler, B * N, R2, Td, s));
   if (A.text_avg_upsample)  // audio lengths: duration (the reference's seq_len = mask.sum), else N
-    RC(run_text_avg_upsample(L.tx, L.txu, L.filler, masked ? L.valid_len : nullptr, B, N, sa->nt, Td, s));
+    RC(run_text_avg_upsample(L.tx, L.txu, L.filler, masked ? L.valid_len : nullptr, B, N, nt, Td, s));
+  return 0;
+}
+
+// xin = [x | cond or 0 | text embedding | 0] of every packed row
+int run_pack(f5_engine* e, const Layout& L, const float* y, const float* step_cond, cudaStream_t s) {
+  const f5_arch& A = e->arch;
   PackParams pp{};
   pp.xin = L.xin_all;
-  pp.B = B;
-  pp.N = N;
+  pp.B = L.B;
+  pp.N = L.N;
   pp.mel = A.mel_dim;
-  pp.Td = Td;
+  pp.Td = A.text_dim;
   pp.Kpad = e->kin;
   pp.packed = L.packed;
-  pp.y = sa->y;
-  pp.step_cond = sa->step_cond;
+  pp.y = y;
+  pp.step_cond = step_cond;
   pp.text = A.text_avg_upsample ? L.txu : L.tx;
-  RC(run_pack_input(pp, s));
+  return run_pack_input(pp, s);
+}
+
+int run_prologue(f5_engine* e, const Layout& L, const f5_sample_args* sa, cudaStream_t s) {
+  const f5_arch& A = e->arch;
+  const int N = L.N, S = L.evals;
+  const bool masked = sa->duration != nullptr;
+  const bool strict = masked && sa->exact_varlen;
+  // small host -> device control data (pageable source: cudaMemcpyAsync stages it before returning).
+  // Per grid interval k (torchdiffeq's fixed-grid solvers): Euler evaluates at t_k and commits y + dt_k * g; midpoint
+  // evaluates at t_k, forms y + half_dt_k * g as the next evaluation's input only, then evaluates at t_k + half_dt_k
+  // and commits y + dt_k * g.  Times are fp32 (the reference builds the grid in the parameter dtype).
+  std::vector<OdeStage> stage;
+  std::vector<float> te;
+  stage.reserve(S);
+  te.reserve(S);
+  for (int k = 0; k < sa->steps; ++k) {
+    const float dt = sa->t[k + 1] - sa->t[k];
+    if (sa->method == 1) {
+      const float half_dt = 0.5f * dt;
+      te.push_back(sa->t[k]);
+      stage.push_back(OdeStage{half_dt, -1});
+      te.push_back(sa->t[k] + half_dt);
+      stage.push_back(OdeStage{dt, k + 1});
+    } else {
+      te.push_back(sa->t[k]);
+      stage.push_back(OdeStage{dt, k + 1});
+    }
+  }
+  RC(check_cuda(cudaMemcpyAsync(L.stage, stage.data(), sizeof(OdeStage) * S, cudaMemcpyHostToDevice, s), "stage h2d"));
+  RC(check_cuda(cudaMemcpyAsync(L.t_dev, te.data(), sizeof(float) * S, cudaMemcpyHostToDevice, s), "t h2d"));
+  RC(check_cuda(cudaMemsetAsync(L.step_ptr, 0, sizeof(int) * 64, s), "step memset"));
+  SampleIo io{sa->y, sa->trajectory, sa->cfg_strength};
+  RC(check_cuda(cudaMemcpyAsync(L.io, &io, sizeof(io), cudaMemcpyHostToDevice, s), "io h2d"));
+  if (masked) RC(set_lengths(e, L, sa->duration, sa->exact_varlen != 0, s));
+  RC(run_rope_table(L.x.rope_cos, L.x.rope_sin, L.x.seq, A.dim_head / 2, s));
+  RC(run_time_embed(e, L, s));  // every evaluation time
+  RC(run_text_embed(e, L, sa->text, sa->nt, masked, strict, s));
+  RC(run_pack(e, L, sa->y, sa->step_cond, s));
   if (sa->trajectory)
-    RC(check_cuda(cudaMemcpyAsync(sa->trajectory, sa->y, sizeof(float) * B * N * A.mel_dim, cudaMemcpyDeviceToDevice, s),
+    RC(check_cuda(cudaMemcpyAsync(sa->trajectory, sa->y, sizeof(float) * L.B * N * A.mel_dim, cudaMemcpyDeviceToDevice, s),
                   "trajectory[0]"));
   return 0;
 }
@@ -933,11 +996,10 @@ int copy_v_out(const f5_engine* e, const Layout& L, const f5_sample_args* sa, cu
   return 0;
 }
 
-// The step graph of this (workspace, shapes, half): from the engine's cache, or captured now on the current device.
-int step_graph(f5_engine* e, const Layout& L, const f5_sample_args* sa, const void* ws,
-               std::shared_ptr<GraphHolder>* out) {
-  const GraphKey key{ws, sa->B, sa->N, L.evals, L.packed, sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1),
-                     e->arch.backbone == kMMDiT ? sa->nt : 0, L.half};
+// The graph of `key`: from the engine's cache, or captured now on the current device.  plan(P) builds the plans the
+// captured work runs, run(P, stream) issues that work.
+template <typename Plan, typename Run>
+int cached_graph(f5_engine* e, const GraphKey& key, Plan&& plan, Run&& run, std::shared_ptr<GraphHolder>* out) {
   std::shared_ptr<GraphHolder> g;
   {
     std::lock_guard<std::mutex> lk(e->mu);
@@ -948,7 +1010,7 @@ int step_graph(f5_engine* e, const Layout& L, const f5_sample_args* sa, const vo
     // Capture outside the engine mutex (thread-local capture mode: concurrent sample() calls capture independently)
     // on a private stream — the caller's stream may be the legacy default stream, which cannot capture.
     StepPlans P;
-    RC(build_step_plans(e, L, sa, P));
+    RC(plan(P));
     cudaStream_t cs;
     RC(check_cuda(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking), "capture stream"));
     if (int brc = check_cuda(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal), "begin capture")) {
@@ -956,7 +1018,7 @@ int step_graph(f5_engine* e, const Layout& L, const f5_sample_args* sa, const vo
       return brc;
     }
     const unsigned long long before = f5_launch_count();
-    const int rc = L.half < 0 ? run_step(e, L, P, cs) : run_body(e, L, P, cs);
+    const int rc = run(P, cs);
     cudaGraph_t graph = nullptr;
     const cudaError_t ce = cudaStreamEndCapture(cs, &graph);
     cudaStreamDestroy(cs);
@@ -981,6 +1043,25 @@ int step_graph(f5_engine* e, const Layout& L, const f5_sample_args* sa, const vo
   }
   *out = std::move(g);
   return 0;
+}
+
+// The step graph of this (workspace, shapes, half)
+int step_graph(f5_engine* e, const Layout& L, const f5_sample_args* sa, const void* ws,
+               std::shared_ptr<GraphHolder>* out) {
+  const GraphKey key{ws, sa->B, sa->N, L.evals, L.packed, sa->duration == nullptr ? 0 : (sa->exact_varlen ? 2 : 1),
+                     e->arch.backbone == kMMDiT ? sa->nt : 0, L.half, 0};
+  return cached_graph(
+      e, key, [&](StepPlans& P) { return build_step_plans(e, L, sa, P); },
+      [&](const StepPlans& P, cudaStream_t cs) { return L.half < 0 ? run_step(e, L, P, cs) : run_body(e, L, P, cs); },
+      out);
+}
+
+// A workspace written by f5_sample no longer holds the text embeddings of an earlier f5_forward call
+void forget_text(f5_engine* e, const void* ws) {
+  std::lock_guard<std::mutex> lk(e->mu);
+  for (size_t i = 0; i < e->text_held.size();)
+    if (e->text_held[i].ws == ws) e->text_held.erase(e->text_held.begin() + i);
+    else ++i;
 }
 
 int check_problem(const char* fn, const f5_sample_args* sa) {
@@ -1024,6 +1105,7 @@ int side_layout(Side& sd, int half) {
 
 // The prologue of one side, then its step graph (use_graph) or its plans
 int side_prepare(Side& sd) {
+  forget_text(sd.e, sd.ws);
   RC(run_prologue(sd.e, sd.L, sd.sa, sd.s));
   if (sd.sa->use_graph) return step_graph(sd.e, sd.L, sd.sa, sd.ws, &sd.g);
   return build_step_plans(sd.e, sd.L, sd.sa, sd.P);
@@ -1235,4 +1317,132 @@ extern "C" int f5_sample_cfg_split(f5_engine* e0, const f5_sample_args* a0, void
   }
   cudaSetDevice(caller_dev);
   return rc;
+}
+
+// -------------------------------------------------------------------------------------------------------------
+// One backbone evaluation (f5_forward): the reference's transformer(x, cond, text, time, mask, ...) operator, with a
+// time per sample.  The layout is f5_sample's with one row of the time and AdaLN tables per sample (evals = B) and
+// L.per_sample set: the norm, gated-residual GEMM (EPI_RESID_SAMPLE) and UNetT time-token kernels read the row of their
+// sample.  Per call:
+//   eager:  time -> t_dev, lengths (with durations), time MLP + AdaLN table of the B times, [text embeddings and rotary
+//           tables unless reuse_text], input pack
+//   graph:  the evaluation up to proj_out (captured once per workspace, shapes, mode and mask given or not; it reads
+//           only the workspace, so new x, cond or times replay it)
+//   eager:  v -> v_out
+// The order is f5_sample's prologue order, for the same reason: the norm kernels fetch their modulation rows before the
+// programmatic-launch wait, so the AdaLN table must be complete before the evaluation's first kernel starts.  The pack
+// kernel, a plain launch, sits between the two and ends only after everything before it.
+namespace {
+
+void forward_layout(const f5_engine* e, Layout& L, void* ws, int B, int N, int nt, int mode) {
+  // cond: un-packed (B rows); CFG: cond | uncond stacked (2B rows); uncond: the unconditional half alone, as one side
+  // of f5_sample_cfg_split computes it
+  plan_layout(e, L, ws, B, N, nt, B, mode == F5_FORWARD_COND ? 0.0f : 1.0f, mode == F5_FORWARD_UNCOND ? 1 : -1);
+  L.per_sample = true;
+}
+
+int forward_check(const f5_forward_args* fa) {
+  if (fa->B <= 0 || fa->N <= 0 || fa->nt <= 0) {
+    set_error("f5_forward: empty problem (B=%d N=%d nt=%d)", fa->B, fa->N, fa->nt);
+    return -1;
+  }
+  if (fa->mode < F5_FORWARD_COND || fa->mode > F5_FORWARD_UNCOND) {
+    set_error("f5_forward: mode must be 0 (cond), 1 (cfg) or 2 (uncond), got %d", fa->mode);
+    return -1;
+  }
+  if (!fa->x || !fa->step_cond || !fa->text || !fa->time || !fa->v_out) {
+    set_error("f5_forward: x, step_cond, text, time and v_out are required");
+    return -1;
+  }
+  return 0;
+}
+
+int forward_run(f5_engine* e, const f5_forward_args* fa, void* ws, size_t ws_bytes, cudaStream_t s) {
+  const f5_arch& A = e->arch;
+  const int B = fa->B, N = fa->N, nt = fa->nt;
+  Layout L;
+  forward_layout(e, L, ws, B, N, nt, fa->mode);
+  if (ws_bytes < L.bytes) {
+    set_error("f5_forward: workspace too small (%zu < %zu)", ws_bytes, L.bytes);
+    return -1;
+  }
+  const bool masked = fa->duration != nullptr;
+  const TextHeld held{ws, B, N, nt, fa->mode, masked ? 1 : 0};
+  {
+    std::lock_guard<std::mutex> lk(e->mu);
+    bool found = false;
+    for (size_t i = 0; i < e->text_held.size();)
+      if (e->text_held[i].ws != ws) {
+        ++i;
+      } else if (fa->reuse_text && e->text_held[i] == held) {
+        found = true;
+        ++i;
+      } else {
+        e->text_held.erase(e->text_held.begin() + i);  // about to be overwritten, or of another problem
+      }
+    if (fa->reuse_text && !found) {
+      set_error("f5_forward: reuse_text, but the workspace holds no text embeddings of this problem (B=%d N=%d nt=%d "
+                "mode %d, durations %s)", B, N, nt, fa->mode, masked ? "given" : "not given");
+      return -1;
+    }
+  }
+  RC(check_cuda(cudaMemcpyAsync(L.t_dev, fa->time, sizeof(float) * B, cudaMemcpyDeviceToDevice, s), "time copy"));
+  if (masked) RC(set_lengths(e, L, fa->duration, false, s));
+  RC(run_time_embed(e, L, s));
+  if (!fa->reuse_text) {
+    RC(run_rope_table(L.x.rope_cos, L.x.rope_sin, L.x.seq, A.dim_head / 2, s));
+    RC(run_text_embed(e, L, fa->text, nt, masked, false, s));
+    std::lock_guard<std::mutex> lk(e->mu);
+    if (e->text_held.size() >= 64) e->text_held.erase(e->text_held.begin());
+    e->text_held.push_back(held);
+  }
+  RC(run_pack(e, L, fa->x, fa->step_cond, s));
+  f5_sample_args sa{};  // the fields build_step_plans reads
+  sa.B = B;
+  sa.N = N;
+  sa.nt = nt;
+  sa.duration = fa->duration;
+  auto run = [&](const StepPlans& P, cudaStream_t cs) { return run_body(e, L, P, cs); };
+  if (fa->use_graph) {
+    const GraphKey key{ws, B, N, L.evals, L.packed, masked ? 1 : 0, A.backbone == kMMDiT ? nt : 0, L.half, 1};
+    std::shared_ptr<GraphHolder> g;
+    RC(cached_graph(e, key, [&](StepPlans& P) { return build_step_plans(e, L, &sa, P); }, run, &g));
+    RC(check_cuda(cudaGraphLaunch(g->exec, s), "graph launch"));
+    count_launch(g->nodes);
+  } else {
+    StepPlans P;
+    RC(build_step_plans(e, L, &sa, P));
+    RC(run(P, s));
+  }
+  // v (this layout's rows: Be samples of seq rows) -> v_out [Be, N, mel], without the UNetT time token
+  const int mel = A.mel_dim, off = A.backbone == kUNetT ? 1 : 0;
+  RC(check_cuda(cudaMemcpy2DAsync(fa->v_out, sizeof(float) * N * mel, L.v + (size_t)off * mel,
+                                  sizeof(float) * L.x.seq * mel, sizeof(float) * N * mel, L.Be,
+                                  cudaMemcpyDeviceToDevice, s),
+                "v_out copy"));
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int f5_engine_graph_count(f5_engine* e) {
+  if (!e) return 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return (int)e->graphs.size();
+}
+
+extern "C" size_t f5_forward_workspace_bytes(const f5_engine* e, int B, int N, int nt, int mode) {
+  Layout L;
+  forward_layout(e, L, nullptr, B, N, nt, mode);
+  return L.bytes;
+}
+
+extern "C" int f5_forward(f5_engine* e, const f5_forward_args* args, void* workspace, size_t ws_bytes,
+                          f5_stream_t stream) {
+  if (!e || !args || !workspace) {
+    set_error("f5_forward: null argument");
+    return -1;
+  }
+  RC(forward_check(args));
+  return forward_run(e, args, workspace, ws_bytes, reinterpret_cast<cudaStream_t>(stream));
 }

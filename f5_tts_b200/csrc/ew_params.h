@@ -17,6 +17,9 @@ struct NormParams {
   long long step_stride;
   int params_static;  // a / b / *step_ptr were not written by the kernel preceding this launch: fetch them before the PDL wait
   const float* skip;  // MODE 3: [rows, D] added to x; the sum is written back to x (x is read-write in that mode)
+  // MODE 4: a / b are read at row ((row / sample_seq) % samples) * step_stride, the modulation row of the row's sample,
+  // instead of the evaluation counter's.  Last, so every other field keeps its parameter offset.
+  int sample_seq, samples;
 };
 
 struct DwConvLnParams {

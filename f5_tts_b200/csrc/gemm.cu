@@ -124,8 +124,21 @@ static const GemmKernel kGemmKernels[] = {
 };
 #undef F5_GEMM_KERNEL
 
+// Engine-internal instantiations that no f5_gemm_args selects: the per-sample gate of f5_forward's gated residual GEMMs
+// (EPI_RESID_SAMPLE), at the widths pick_tile chooses from for EPI_RESID.  The engine plans such a GEMM as EPI_RESID and
+// then switches the plan's epilogue, so the width is the one f5_sample runs the same problem with.
+// tests/test_gpu_gemm_resid_sample.py checks each entry element by element against per-sample EPI_RESID launches.
+template <int BN>
+constexpr GemmKernel sample_gate_kernel() {
+  return GemmKernel{BN, EPI_RESID_SAMPLE, ACT_NONE, false, gemm_wgmma_kernel<BN, EPI_RESID_SAMPLE, ACT_NONE, false>};
+}
+static const GemmKernel kGemmSampleKernels[] = {sample_gate_kernel<128>(), sample_gate_kernel<192>(),
+                                                sample_gate_kernel<256>()};
+
 static const GemmKernel* find_kernel(int bn, int epi, int act, bool conv) {
   for (const GemmKernel& k : kGemmKernels)
+    if (k.bn == bn && k.epi == epi && k.act == act && k.conv == conv) return &k;
+  for (const GemmKernel& k : kGemmSampleKernels)
     if (k.bn == bn && k.epi == epi && k.act == act && k.conv == conv) return &k;
   return nullptr;
 }
@@ -151,13 +164,17 @@ int configure_kernels() {
   const int dev = current_device();
   std::lock_guard<std::mutex> lk(g_dev_mu);
   if (g_dev[dev].configured) return 0;
-  for (const GemmKernel& k : kGemmKernels) {
-    if (int rc = check_cuda(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 (int)gemm_smem_bytes(k.bn)),
-                            "cudaFuncSetAttribute(gemm smem)"))
-      return rc;
-    cudaFuncSetAttribute(k.fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
-  }
+  auto setup = [](const GemmKernel& k) {
+    const int rc = check_cuda(cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                   (int)gemm_smem_bytes(k.bn)),
+                              "cudaFuncSetAttribute(gemm smem)");
+    if (rc == 0) cudaFuncSetAttribute(k.fn, cudaFuncAttributePreferredSharedMemoryCarveout, 100);
+    return rc;
+  };
+  for (const GemmKernel& k : kGemmKernels)
+    if (int rc = setup(k)) return rc;
+  for (const GemmKernel& k : kGemmSampleKernels)
+    if (int rc = setup(k)) return rc;
   if (int rc = attn_configure()) return rc;
   g_dev[dev].configured = true;
   return 0;
@@ -384,7 +401,7 @@ int gemm_plan(GemmPlan* pl, const void* A, const void* W, const f5_gemm_args* a)
 
 extern "C" {
 
-int f5_version(void) { return 109; }
+int f5_version(void) { return 110; }
 const char* f5_last_error(void) { return f5::g_err; }
 unsigned long long f5_launch_count(void) { return f5::g_launches.load(); }
 

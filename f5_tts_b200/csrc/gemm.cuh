@@ -71,16 +71,21 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
   // exactly as when they compared with p.n_out directly.
   auto n_end = [&]() { return CONV ? n0 + p.conv_g : p.n_out; };
   constexpr bool NORM = EPI == EPI_QKV_NORM_ROPE || EPI == EPI_QKV_NORM_ROPE_DH128;
+  // per-sample gate rows (EPI_RESID_SAMPLE): each of the thread's two rows may lie in another sample
+  constexpr bool PS = EPI == EPI_RESID_SAMPLE;
+  constexpr bool RESID = EPI == EPI_RESID || PS;
   constexpr bool QKV = EPI == EPI_QKV_ROPE || EPI == EPI_QKV_ROPE_DH128 || NORM;
   // head width of the QKV epilogues (columns of one q, k or v head)
   constexpr int DH = (EPI == EPI_QKV_ROPE_DH128 || EPI == EPI_QKV_NORM_ROPE_DH128) ? 128 : 64;
   constexpr int LOG_DH = DH == 128 ? 7 : 6;
   // chunk width: the widest whose loads fit beside the BN / 2 accumulators without spilling (ptxas caps a 288-thread
   // CTA at 168 registers per thread).  QKV_NORM_ROPE adds its bias before the chunks, which frees the bias registers.
+  // RESID_SAMPLE keeps a second row of gates: half the RESID chunk at 128 and 256.
   constexpr int CW = NORM ? (BN <= 128 ? 64 : BN == 192 ? 32 : 8)
+                   : PS   ? (BN == 256 ? 8 : 32)
                    : BN <= 128 ? (QKV ? 32 : 64)
                      : BN == 192 ? (QKV ? 16 : 32)
-                                 : (EPI == EPI_F16 ? 32 : EPI == EPI_RESID ? 16 : 8);
+                                 : (EPI == EPI_F16 ? 32 : RESID ? 16 : 8);
   constexpr int J = CW / 8;  // column pairs of one thread in a chunk
   bool in[2], valid[2];
   long long grow[2];
@@ -96,7 +101,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
       pos[h] = int(grow[h] % p.seq);
       if (p.row_len != nullptr) valid[h] = pos[h] < p.row_len[grow[h] / p.seq];
     }
-    if (EPI == EPI_RESID) in[h] = in[h] && valid[h];  // masked rows keep their residual
+    if (RESID) in[h] = in[h] && valid[h];  // masked rows keep their residual
+  }
+  const float* gate_row[2] = {gate, gate};
+  if (PS && gate != nullptr) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (in[h]) gate_row[h] = gate + (long long)((grow[h] / p.gate_seq) % p.gate_samples) * p.gate_step_stride;
   }
   // qk_norm shuffles within quads: every lane of the warp has to reach them, so no lane leaves early
   if (!NORM && !in[0] && !in[1]) return;
@@ -136,12 +147,13 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
     }
     if (NORM && !in[0] && !in[1]) continue;
     // ---- loads ----
-    float2 b[J], g[J];
+    float2 b[J], g[J], gs[2][J];  // gs: PS only, the gates of rows row0 and row0 + 8
 #pragma unroll
     for (int j = 0; j < J; ++j) {
       const int nc = nb + 8 * j + c2;
       b[j] = make_float2(0.0f, 0.0f);
       g[j] = make_float2(1.0f, 1.0f);
+      gs[0][j] = gs[1][j] = g[j];
       if (nc >= n_end()) continue;
       const bool pair_ok = nc + 1 < n_end();
       if (!NORM && p.bias != nullptr) {
@@ -151,6 +163,14 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
       if (EPI == EPI_RESID && gate != nullptr) {
         g[j].x = gate[nc];
         if (pair_ok) g[j].y = gate[nc + 1];
+      }
+      if (PS && gate != nullptr) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!in[h]) continue;
+          gs[h][j].x = gate_row[h][nc];
+          if (pair_ok) gs[h][j].y = gate_row[h][nc + 1];
+        }
       }
     }
     bool rope = false, nrm = false;
@@ -179,7 +199,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
       }
     }
     float2 x[2][J];
-    if (EPI == EPI_RESID) {
+    if (RESID) {
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -250,15 +270,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float* acc, i
               if (pair_ok) o2[1] = __float2half_rn(v1);
             }
           }
-        } else if (EPI == EPI_RESID) {
+        } else if (RESID) {
           float* o = p.resid + grow[h] * p.ldo + nc;
           float2 xv = x[h][j];
+          const float2 gg = PS ? gs[h][j] : g[j];
           if (pair_ok) {
-            xv.x += g[j].x * v0;
-            xv.y += g[j].y * v1;
+            xv.x += gg.x * v0;
+            xv.y += gg.y * v1;
             *reinterpret_cast<float2*>(o) = xv;
           } else {
-            o[0] = xv.x + g[j].x * v0;
+            o[0] = xv.x + gg.x * v0;
           }
         }
       }
@@ -352,6 +373,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const float* gate = nullptr;
     if (EPI == EPI_RESID && p.gate != nullptr)
       gate = p.gate + (p.step_ptr ? (long long)(*p.step_ptr) : 0) * p.gate_step_stride;
+    if (EPI == EPI_RESID_SAMPLE) gate = p.gate;  // the row of each output row's sample is picked in the epilogue
     float acc[BN / 2];
     uint32_t it = 0;
     auto release = [&](int s) {

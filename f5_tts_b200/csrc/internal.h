@@ -97,6 +97,9 @@ int run_silu_to_half(const float* in, __half* out, long long n, cudaStream_t s);
 int run_rope_table(float* cs, float* sn, int seq, int half, cudaStream_t s);
 int run_prepend_time_token(float* dst, const float* src, const float* t_emb, const int* step_ptr, int N, int D,
                            long long rows_out, cudaStream_t s);
+// f5_forward: row 0 of sample b is t_emb[b % samples] (each sample's own time)
+int run_prepend_time_token_per_sample(float* dst, const float* src, const float* t_emb, int samples, int N, int D,
+                                      long long rows_out, cudaStream_t s);
 int run_concat_half(const float* x, const float* skip, __half* out, long long rows, int D, cudaStream_t s);
 
 // ---- FFT tables and the Vocos kernels outside the GEMMs (ops.cu) ----

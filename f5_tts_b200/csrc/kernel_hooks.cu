@@ -14,6 +14,23 @@ extern "C" {
 
 const char* f5k_last_error() { return f5_last_error(); }
 
+// EPI_RESID_SAMPLE, the engine-internal gated residual epilogue of f5_forward: the f5_gemm problem `a` (F5_EPI_RESID,
+// gate = row 0 of a table of gate_step_stride floats per row, step_ptr NULL) with the gate row of each output row's
+// sample, (row / gate_seq) % gate_samples
+int f5k_gemm_resid_sample(const void* A, const void* W, const f5_gemm_args* a, int gate_seq, int gate_samples,
+                          void* s) {
+  if (!a || a->epi != F5_EPI_RESID || !a->gate || a->step_ptr || gate_seq <= 0 || gate_samples <= 0) {
+    set_error("gemm_resid_sample: needs F5_EPI_RESID with a gate table, no step_ptr, gate_seq and gate_samples > 0");
+    return -1;
+  }
+  GemmPlan pl;
+  if (int rc = gemm_plan(&pl, A, W, a)) return rc;
+  pl.epi = EPI_RESID_SAMPLE;
+  pl.p.gate_seq = gate_seq;
+  pl.p.gate_samples = gate_samples;
+  return gemm_run(pl, st(s));
+}
+
 int f5k_row_norm(int mode, const float* x, void* out, int rows, int D, float eps, const float* a, const float* b,
                  const int* step_ptr, long long step_stride, int params_static, void* s) {
   NormParams p{};

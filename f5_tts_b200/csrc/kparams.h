@@ -18,6 +18,10 @@ enum : int {
   // f5_gemm_args.dim_head = 128.
   EPI_QKV_ROPE_DH128 = 5,
   EPI_QKV_NORM_ROPE_DH128 = 6,
+  // EPI_RESID with the gate row of each output row's sample: gate + ((row / gate_seq) % gate_samples) *
+  // gate_step_stride.  Engine-internal (f5_forward, gemm.cu: kGemmSampleKernels), so the kernels of f5_sample keep
+  // their step-indexed gate.
+  EPI_RESID_SAMPLE = 7,
 };
 
 struct GemmParams {
@@ -50,6 +54,10 @@ struct GemmParams {
   // parameter offsets.
   const float* q_norm;
   const float* k_norm;
+  // EPI_RESID_SAMPLE: rows per sample, and the number of gate rows (the samples of the call; the conditional and
+  // unconditional rows of a sample share one).  Last, so every other field keeps its parameter offset.
+  int gate_seq;
+  int gate_samples;
 };
 
 constexpr int kBM = 128;

@@ -55,7 +55,12 @@ int run_row_norm(int mode, const NormParams& p, cudaStream_t s) {
   constexpr int wpb = 4;
   PdlLaunch L(dim3((p.rows + wpb - 1) / wpb), dim3(32 * wpb), 0, s);
   cudaError_t ce;
-  if (mode == 0) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<0>, p);
+  if (mode == 4 && (p.samples <= 0 || p.sample_seq <= 0)) {
+    set_error("row_norm: mode 4 needs samples > 0 and sample_seq > 0 (got %d, %d)", p.samples, p.sample_seq);
+    return -1;
+  }
+  if (mode == 4) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<4>, p);
+  else if (mode == 0) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<0>, p);
   else if (mode == 1) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<1>, p);
   else if (mode == 2) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<2>, p);
   else if (mode == 3 && p.skip != nullptr) ce = cudaLaunchKernelEx(&L.cfg, row_norm_kernel<3>, p);
@@ -188,6 +193,17 @@ int run_prepend_time_token(float* dst, const float* src, const float* t_emb, con
     return rc;
   count_launch();
   return check_launch("prepend_time_token_kernel");
+}
+
+int run_prepend_time_token_per_sample(float* dst, const float* src, const float* t_emb, int samples, int N, int D,
+                                      long long rows_out, cudaStream_t s) {
+  PdlLaunch L(dim3((unsigned)rows_out), dim3(256), 0, s);
+  if (int rc = check_cuda(cudaLaunchKernelEx(&L.cfg, prepend_time_token_sample_kernel, dst, src, t_emb, samples, N, D,
+                                             rows_out),
+                          "prepend_time_token_sample launch"))
+    return rc;
+  count_launch();
+  return check_launch("prepend_time_token_sample_kernel");
 }
 
 int run_concat_half(const float* x, const float* skip, __half* out, long long rows, int D, cudaStream_t s) {

@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 import threading
 from typing import Callable, Optional
 
@@ -311,8 +312,25 @@ class _Backbone(nn.Module):
                 pass
 
     def clear_cache(self):
-        """Text embeddings are recomputed inside every engine call; nothing is cached across calls."""
+        """Release this thread's operator state: the workspaces of `forward` and the text embeddings a cache=True call
+        keeps (the reference clears its per-thread text cache the same way, dit.py:316-317).  sample() recomputes its
+        text embeddings in every engine call and keeps nothing across calls."""
+        local = self.__dict__.get("_op_local")
+        if local is not None:
+            local.states = {}
         return None
+
+    def _op_states(self) -> dict:
+        """This thread's operator state, (cache, device, stream) -> {"ws", "engine", "key"}.  The threading.local is made
+        on first use and kept out of the module's attributes, as the reference keeps its text cache (dit.py:237-243)."""
+        local = self.__dict__.get("_op_local")
+        if local is None:
+            with self._engine_lock:
+                local = self.__dict__.setdefault("_op_local", threading.local())
+        states = getattr(local, "states", None)
+        if states is None:
+            states = local.states = {}
+        return states
 
     def _ws_acquire(self, nbytes: int, device, stream: int) -> torch.Tensor:
         """Scratch for one engine call, from a pool keyed on (device, stream).  Concurrent sample() calls (the reference
@@ -351,7 +369,11 @@ class _Backbone(nn.Module):
                                exact_varlen, method)
 
     def _run_local(self, y, step_cond, text, t_grid, duration, cfg_strength, trajectory=None, v_out=None,
-                   use_graph=True, exact_varlen=False, method="euler"):
+                   use_graph=True, exact_varlen=False, method="euler", forward=None):
+        """One engine call on the model's own device.  forward=(mode, cache): a backbone-operator call instead, one
+        f5_forward evaluation at the per-sample times t_grid (fp32 [B]) written to v_out."""
+        if forward is not None:
+            return self._forward_local(y, step_cond, text, t_grid, duration, v_out, *forward)
         st = self.engine()
         L = _lib.lib()
         B, N, mel = y.shape
@@ -380,22 +402,70 @@ class _Backbone(nn.Module):
     @torch.no_grad()
     def forward(self, x, cond, text, time, mask=None, drop_audio_cond=False, drop_text=False, cfg_infer=False,
                 cache=False):
-        """Flow prediction: float[b | 2b, n, mel].  cfg_infer packs (cond, uncond) on the batch axis."""
+        """Flow prediction: float[b | 2b, n, mel], each sample at its own time.  One f5_forward call on the model's
+        device (the CFG and sample splits do not apply), replayed from a CUDA graph after its first call at these shapes.
+
+        time: a float, a 0-d tensor, [1] (every sample at that time) or [b] (the reference's float["b"]); any other
+        shape raises ValueError.  cfg_infer packs (cond, uncond) on the batch axis; drop_audio_cond = drop_text = True
+        returns the unconditional flow.
+        cache=True (the reference's semantics, dit.py:284-311): this thread's first call computes the text embeddings
+        and later calls reuse them until clear_cache(), even when `text` changes.  A call at another b, n, text length,
+        mode or with / without `mask` computes them again.  cache=False computes them in every call."""
         if drop_audio_cond != drop_text:
             raise NotImplementedError("only the joint (audio+text) drop used by CFG inference is built")
         B, N, mel = x.shape
         dev = x.device
-        t0 = float(time.reshape(-1)[0]) if torch.is_tensor(time) else float(time)
-        y = x.detach().float().contiguous().clone()
-        sc = cond.detach().float().contiguous()
+        t = forward_times(time, B, dev)
+        mode = _lib.FORWARD_CFG if cfg_infer else (_lib.FORWARD_UNCOND if drop_text else _lib.FORWARD_COND)
         duration = None if mask is None else mask.sum(dim=1).to(torch.int32).contiguous()
-        packed = cfg_infer or drop_text
-        v = torch.empty((2 * B if packed else B, N, mel), device=dev, dtype=torch.float32)
-        self._run_local(y, sc, text.to(torch.int64).contiguous(), [t0, t0 + 1.0], duration, 1.0 if packed else 0.0,
-                        None, v, use_graph=False)
-        if cfg_infer:
-            return v.to(x.dtype)
-        return (v[B:] if drop_text else v).to(x.dtype)
+        v = torch.empty((2 * B if mode == _lib.FORWARD_CFG else B, N, mel), device=dev, dtype=torch.float32)
+        self._run_local(x.detach().float().contiguous(), cond.detach().float().contiguous(),
+                        text.to(torch.int64).contiguous(), t, duration, 0.0 if mode == _lib.FORWARD_COND else 1.0, None,
+                        v, forward=(mode, bool(cache)))
+        return v.to(x.dtype)
+
+    def _forward_local(self, x, step_cond, text, t, duration, v_out, mode, cache):
+        """f5_forward on this thread's workspace for (cache, device, stream).  Its address keys the graph, and with
+        cache=True it holds the text embeddings the next call at the same problem reuses."""
+        B, N, _ = x.shape
+        dev = x.device
+        nt = text.shape[1]
+        st = self.engine()
+        handle = st["handle"]
+        L = _lib.lib()
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        states = self._op_states()
+        need = L.f5_forward_workspace_bytes(handle, B, N, nt, mode)
+        op = states.get((cache, dev, stream))
+        # a re-packed engine (weights changed) holds no text embeddings and no graphs of the old one
+        if op is None or op["engine"] is not st or op["ws"].numel() < need:
+            op = states[(cache, dev, stream)] = {"ws": torch.empty(need, dtype=torch.uint8, device=dev), "engine": st,
+                                                 "key": None}
+        key = (B, N, nt, mode, duration is not None)
+        a = _lib.ForwardArgs()
+        a.B, a.N, a.nt = B, N, nt
+        a.x, a.step_cond, a.text, a.time = x.data_ptr(), step_cond.data_ptr(), text.data_ptr(), t.data_ptr()
+        a.duration = duration.data_ptr() if duration is not None else None
+        a.mode, a.v_out, a.use_graph = mode, v_out.data_ptr(), 1
+        a.reuse_text = 1 if (cache and op["key"] == key) else 0
+        op["key"] = None  # until the call has succeeded
+        with torch.cuda.device(dev):
+            _lib.check(L.f5_forward(handle, C.byref(a), op["ws"].data_ptr(), op["ws"].numel(), stream), "f5_forward")
+        op["key"] = key if cache else None
+
+
+def forward_times(time, B: int, device) -> torch.Tensor:
+    """The operator's `time` as fp32 [B] on `device`: a Python number, a 0-d tensor, a [1] tensor (every sample at that
+    time) or a [B] tensor (one time per sample).  Any other shape raises ValueError."""
+    if isinstance(time, numbers.Real):
+        return torch.full((B,), float(time), dtype=torch.float32, device=device)
+    if not torch.is_tensor(time):
+        raise ValueError(f"time must be a number or a tensor, got {type(time).__name__}")
+    if time.dim() == 0 or tuple(time.shape) == (1,):
+        time = time.reshape(1).expand(B)
+    elif tuple(time.shape) != (B,):
+        raise ValueError(f"time must be a scalar, [1] or [b] = [{B}], got shape {tuple(time.shape)}")
+    return time.to(device=device, dtype=torch.float32).contiguous()
 
 
 class DiT(_Backbone):

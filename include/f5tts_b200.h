@@ -273,6 +273,37 @@ int f5_sample_cfg_split(f5_engine* e0, const f5_sample_args* a0, void* ws0, size
 /* workspace of either side of f5_sample_cfg_split (nfe as for f5_sample_workspace_bytes).  Since f5_version() 109. */
 size_t f5_sample_cfg_split_workspace_bytes(const f5_engine* e, int B, int N, int nt, int nfe);
 
+/* One backbone evaluation: the reference's operator transformer(x, cond, text, time, mask, drop_audio_cond, drop_text,
+ * cfg_infer, cache) (backbones/dit.py:319-370, unett.py:244-307, mmdit.py:198-246) with a time per sample, for samplers
+ * outside f5_sample (another ODE method, a solver of the caller's, samples at different times).  Since f5_version() 110.
+ *   mode F5_FORWARD_COND: the conditional flow [B, N, mel]; F5_FORWARD_CFG: cond rows then uncond rows [2B, N, mel]
+ *   (cfg_infer=True); F5_FORWARD_UNCOND: the unconditional flow [B, N, mel] (drop_audio_cond = drop_text = True).
+ *   Each sample's time embedding, AdaLN rows and UNetT time token come from its own time[b]; the cond and uncond rows of
+ *   a sample share them.
+ *   use_graph: the evaluation runs as one CUDA graph, captured once per (workspace, B, N, nt for MMDiT, mode, duration
+ *   given or not) and replayed.  Before it, outside the graph, x and step_cond are packed into the workspace's input
+ *   operand and the time embedding and AdaLN rows of `time` are computed there, so new values replay the same graph.
+ *   reuse_text: skip the text embeddings and rotary tables and use those the previous f5_forward call on this workspace
+ *   computed, even if `text` changed since (the reference's cache=True).  That call must have had the same B, N, nt, mode
+ *   and durations given or not, and no f5_sample call may have used the workspace since; otherwise the call fails. */
+enum { F5_FORWARD_COND = 0, F5_FORWARD_CFG = 1, F5_FORWARD_UNCOND = 2 };
+typedef struct {
+  int B, N, nt;
+  const float* x;          /* device fp32 [B, N, mel]: the noisy state */
+  const float* step_cond;  /* device fp32 [B, N, mel]: the masked cond audio */
+  const long long* text;   /* device int64 [B, nt], padded with -1 */
+  const int* duration;     /* device int32 [B] = mask.sum(1) (the reference's batched mask semantics), or NULL */
+  const float* time;       /* device fp32 [B] */
+  int mode;                /* F5_FORWARD_* */
+  float* v_out;            /* device fp32 [2B, N, mel] for F5_FORWARD_CFG, else [B, N, mel] */
+  int use_graph;
+  int reuse_text;
+} f5_forward_args;
+size_t f5_forward_workspace_bytes(const f5_engine* e, int B, int N, int nt, int mode);
+/* number of captured CUDA graphs the engine holds (f5_sample and f5_forward; at most 16).  Since f5_version() 110. */
+int f5_engine_graph_count(f5_engine* e);
+int f5_forward(f5_engine* e, const f5_forward_args* args, void* workspace, size_t ws_bytes, f5_stream_t stream);
+
 /* algorithmic FLOPs of one f5_sample call making nfe backbone evaluations (SURVEY.md §8d formula) — used by bench.py
  * for the roofline */
 double f5_sample_flops(const f5_engine* e, int B, int N, int nfe, float cfg_strength);
