@@ -148,6 +148,11 @@ def lib():
         L.f5_attention_dh.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p]
         L.f5_attention_joint.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                          c_void_p, c_void_p, c_int, c_float, c_void_p]
+        L.f5_attention_qwg.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_int,
+                                       c_void_p]
+        L.f5_attention_joint_qwg.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
+                                             c_void_p, c_void_p, c_int, c_float, c_int, c_void_p]
+        L.f5_attention_qwg_choice.argtypes = [c_int, c_int, c_int, c_int]
         L.f5_row_norm.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p]
         L.f5_mel_spectrogram.argtypes = [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p]
         L.f5_vocos_workspace_bytes.argtypes = [c_int, c_int]
@@ -177,7 +182,8 @@ def lib():
         L.f5_forward_workspace_bytes.restype = c_size_t
         L.f5_engine_graph_count.argtypes = [c_void_p]
         L.f5_engine_graph_count.restype = c_int
-        for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_attention_joint", "f5_row_norm", "f5_mel_spectrogram",
+        for name in ("f5_gemm", "f5_gemm_tile", "f5_attention", "f5_attention_dh", "f5_attention_joint", "f5_attention_qwg", "f5_attention_joint_qwg",
+                     "f5_row_norm", "f5_mel_spectrogram",
                      "f5_vocos_decode",
                      "f5_vocos_decode_varlen", "f5_engine_create", "f5_sample", "f5_sample_cfg_split", "f5_forward"):
             getattr(L, name).restype = c_int
@@ -201,7 +207,8 @@ EXPORTED_SYMBOLS = [
     "f5_vocos_workspace_bytes", "f5_vocos_decode", "f5_vocos_decode_varlen", "f5_engine_create", "f5_engine_destroy",
     "f5_sample_workspace_bytes", "f5_sample", "f5_sample_flops", "f5_attention_joint", "f5_sample_workspace_bytes_nt",
     "f5_sample_flops_nt", "f5_sample_cfg_split", "f5_sample_cfg_split_workspace_bytes", "f5_forward",
-    "f5_forward_workspace_bytes", "f5_engine_graph_count",
+    "f5_forward_workspace_bytes", "f5_engine_graph_count", "f5_attention_qwg", "f5_attention_joint_qwg",
+    "f5_attention_qwg_choice",
 ]
 
 # Test-only library: the same objects plus one extern "C" wrapper per kernel launcher (csrc/kernel_hooks.cu), used by

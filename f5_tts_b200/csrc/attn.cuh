@@ -1,12 +1,14 @@
 // Non-causal flash-attention forward on wgmma for dim_head DH = 64 or 128 (reference: model/modules.py:471-556,
 // F.scaled_dot_product_attention(q, k, v, attn_mask=None | key mask), scale 1/sqrt(DH)).
 //
-// One CTA = one (sample, head, 128-query block).  q/k/v are read in place from the fused QKV projection output
-// [Be*seq, 3*inner] (fp16) through ONE 3-D TMA tensor map (cols, seq rows, sample): no head-split transpose ever touches
-// HBM, and rows past the end of a sample are zero-filled by TMA instead of leaking the next sample.  A 128B-swizzled box
+// One CTA = one (sample, head, block of 64 QWG queries), QWG = 2 or (DH = 64 only) 4 consumer warpgroups.  q/k/v are
+// read in place from the fused QKV projection output [Be*seq, 3*inner] (fp16) through ONE 3-D TMA tensor map (cols,
+// seq rows, sample): no head-split transpose ever touches HBM, and rows past the end of a sample are zero-filled by
+// TMA instead of leaking the next sample.  A 128B-swizzled box
 // is at most 64 fp16 wide, so a 128-row tile of a head is DH / 64 boxes of 128 x 64 (16 KB each), one after the other.
-// Warp roles (288 threads): warps 0..7 = two consumer warpgroups, warpgroup g owns query rows [64 g, 64 g + 64);
-// warp 8 = TMA producer (Q once, then a kAttnStages-deep ring of K and V tiles of 128 keys).
+// Warp roles: warps 0..4 QWG - 1 = QWG consumer warpgroups, warpgroup g owns query rows [64 g, 64 g + 64).  The TMA
+// loads (Q once, then a kAttnStages-deep ring of K and V tiles of 128 keys) come from warp 8, a producer warp of its
+// own, at QWG = 2 (288 threads), and from consumer warp 0 at QWG = 4 (512 threads; see attn_threads).
 //   S = Q K^T   : wgmma m64n128k16 x DH / 16, both operands K-major in shared memory, fp32 in registers
 //   softmax     : online max / sum in fp32 on the accumulator fragment (a row is spread over the four threads of a
 //                 quad: two shuffles per row max); exponentials with MUFU.EX2 in log2 units
@@ -14,7 +16,9 @@
 //                 wgmma's register A operand, so P never touches shared memory — times V consumed MN-major straight
 //                 from its TMA layout (wgmma m64nDHk16, transposed B; at DH = 128 the two 64-column boxes of V are the
 //                 two 64-wide MN blocks of the operand, kAttnTile bytes apart)
-// The two warpgroups run independently, so one's exponentials overlap the other's tensor-core work.
+// The warpgroups run independently, so one's exponentials overlap another's tensor-core work.  Every query row goes
+// through the same instructions whatever QWG is, so both widths give the same output bit for bit; QWG = 4 (one CTA
+// per SM) puts twice the rows on each SM's tensor cores and halves the K/V loads per query.
 #pragma once
 #include "common.cuh"
 #include "kparams.h"
@@ -33,17 +37,21 @@ __device__ __forceinline__ float ex2_approx(float x) {  // one MUFU.EX2; -inf ->
 // blocks [0, jp.q_blocks_a) are audio, the rest text; each writes its own segment's output.  The producer streams the
 // audio key tiles, then the text key tiles, through the same ring; the tail of each segment is masked on its own, so
 // every tile still holds at least one valid key.  A text segment with no valid keys contributes no tile.
-template <int DH, bool JOINT>
+template <int DH, bool JOINT, int QWG>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CUtensorMap* tmC, const AttnParams& p,
                                               const AttnJointParams& jp) {
   static_assert(DH == 64 || DH == 128, "head width");
+  static_assert(QWG == 2 || (QWG == 4 && DH == 64), "4 query warpgroups only at head width 64 (register budget)");
   constexpr int BOXES = DH / 64;                   // 64-column TMA boxes per tile row
   constexpr uint32_t TILE = kAttnTile * BOXES;     // one 128-row tile of q, k or v
+  constexpr int QBOXES = QWG / 2;                  // 128-row tiles of q
+  constexpr int BQ = 64 * QWG;                     // query rows per CTA
+  constexpr int PRODUCER = QWG == 2 ? 8 : 0;       // warp that issues the TMA loads (at QWG = 4 a consumer warp)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - smem_u32(smem_raw));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + TILE;                         // kAttnStages tiles
+  uint8_t* sQ = smem;                              // QBOXES tiles: warpgroup g's 64 rows start at g * 8 KB
+  uint8_t* sK = sQ + QBOXES * TILE;                // kAttnStages tiles
   uint8_t* sV = sK + kAttnStages * TILE;           // kAttnStages tiles
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kAttnStages * TILE);
   uint64_t* q_full = bars;                         // [1]
@@ -55,23 +63,23 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CU
   const int warp = threadIdx.x >> 5;
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   bool text_q = false;  // JOINT: this CTA's queries are text rows
-  int q0 = qb * kAttnBQ;
+  int q0 = qb * BQ;
   if constexpr (JOINT) {
     text_q = qb >= jp.q_blocks_a;
-    if (text_q) q0 = (qb - jp.q_blocks_a) * kAttnBQ;
+    if (text_q) q0 = (qb - jp.q_blocks_a) * BQ;
   }
   const CUtensorMap* tmQ = text_q ? tmC : tmQKV;
   const int col_q = h * DH, col_k = p.inner + h * DH, col_v = 2 * p.inner + h * DH;
 
-  if (warp == 8 && elect_one()) {
+  if (warp == PRODUCER && elect_one()) {
     tma_prefetch_desc(tmQKV);
     if constexpr (JOINT) tma_prefetch_desc(tmC);
     mbar_init(q_full, 1);
     for (int s = 0; s < kAttnStages; ++s) {
       mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], 8);  // one arrival per consumer warp
+      mbar_init(&k_empty[s], 4 * QWG);  // one arrival per consumer warp
       mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], 8);
+      mbar_init(&v_empty[s], 4 * QWG);
     }
     fence_mbar_init();
   }
@@ -88,7 +96,27 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CU
     n_kv += (kv_len_c + kAttnBKV - 1) / kAttnBKV;
   }
 
-  if (warp == 8) {
+  // QWG = 4 (BOXES = 1): K and V of key tile j into ring slot j % kAttnStages, once that slot is free
+  auto load_kv = [&](int j) {
+    const int s = j % kAttnStages;
+    bool text_kv = false;
+    if constexpr (JOINT) text_kv = j >= n_kv_a;
+    const CUtensorMap* tmKV = text_kv ? tmC : tmQKV;
+    const int k0 = (text_kv ? j - n_kv_a : j) * kAttnBKV;
+    mbar_expect_tx(&k_full[s], TILE);
+    tma_load_3d(sK + s * TILE, tmKV, &k_full[s], col_k, k0, b);
+    mbar_expect_tx(&v_full[s], TILE);
+    tma_load_3d(sV + s * TILE, tmKV, &v_full[s], col_v, k0, b);
+  };
+  if constexpr (QWG == 4) {
+    if (warp == PRODUCER && lane_id() == 0) {  // q tiles that hold no query row of the sample are not loaded
+      const int seq_q = text_q ? jp.seq_c : p.seq;
+      const int nq = min(QBOXES, (seq_q - q0 + 127) / 128);
+      mbar_expect_tx(q_full, nq * TILE);
+      for (int t = 0; t < nq; ++t) tma_load_3d(sQ + t * TILE, tmQ, q_full, col_q, q0 + 128 * t, b);
+      for (int j = 0; j < min(n_kv, kAttnStages); ++j) load_kv(j);  // the empty ring; later tiles: consumer loop
+    }
+  } else if (warp == PRODUCER) {
     if (elect_one()) {
       mbar_expect_tx(q_full, TILE);
 #pragma unroll
@@ -137,6 +165,22 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CU
   const int r = 64 * g + 16 * (warp & 3) + (lane >> 2);
   const int c2 = 2 * (lane & 3);
   const uint64_t qdesc = make_wgmma_desc_sw128(smem_u32(sQ + g * (64 * 128)));
+  if constexpr (QWG > 2) {
+    const int seq_q = text_q ? jp.seq_c : p.seq;
+    if (q0 + 64 * g >= seq_q) {  // no query row of the sample: no MMA, but every ring slot is waited on and released
+      for (int j = 0; j < n_kv; ++j) {
+        const int s = j % kAttnStages;
+        const uint32_t ph = (j / kAttnStages) & 1;
+        mbar_wait(&k_full[s], ph);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&k_empty[s]);
+        mbar_wait(&v_full[s], ph);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&v_empty[s]);
+      }
+      return;
+    }
+  }
   float o[DH / 2];
 #pragma unroll
   for (int i = 0; i < DH / 2; ++i) o[i] = 0.0f;
@@ -145,6 +189,22 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CU
   for (int j = 0; j < n_kv; ++j) {
     const int s = j % kAttnStages;
     const uint32_t ph = (j / kAttnStages) & 1;
+    if constexpr (QWG == 4) {
+      // warp 0 refills the slot of tile j - 1 with tile j + 2 once every warp has released it.  Warpgroup 0 itself
+      // released it last iteration, and the other warpgroups may run up to two tiles ahead of it, so in steady state
+      // it finds the slot free and the load is issued two tiles before it is needed.  (Warpgroup 0 always has a
+      // query row, so it never takes the no-MMA path above.)
+      if (warp == PRODUCER && j >= 1 && j + 2 < n_kv) {
+        if (lane == 0) {
+          const int sf = (j + 2) % kAttnStages;
+          const uint32_t phf = ((j - 1) / kAttnStages) & 1;
+          mbar_wait(&k_empty[sf], phf);
+          mbar_wait(&v_empty[sf], phf);
+          load_kv(j + 2);
+        }
+        __syncwarp();
+      }
+    }
     int kv_rem = kv_len - j * kAttnBKV;  // valid keys in this tile (>= 1)
     if constexpr (JOINT) {
       if (j >= n_kv_a) kv_rem = kv_len_c - (j - n_kv_a) * kAttnBKV;
@@ -240,17 +300,17 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap* tmQKV, const CU
   }
 }
 
-template <int DH>
-__global__ void __launch_bounds__(kAttnThreads, 1)
+template <int DH, int QWG>
+__global__ void __launch_bounds__(attn_threads(QWG), 1)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnParams p) {
-  attn_fwd_body<DH, false>(&tmQKV, &tmQKV, p, AttnJointParams{});
+  attn_fwd_body<DH, false, QWG>(&tmQKV, &tmQKV, p, AttnJointParams{});
 }
 
-template <int DH>
-__global__ void __launch_bounds__(kAttnThreads, 1)
+template <int DH, int QWG>
+__global__ void __launch_bounds__(attn_threads(QWG), 1)
 attn_joint_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmC,
                         const AttnParams p, const AttnJointParams jp) {
-  attn_fwd_body<DH, true>(&tmQKV, &tmC, p, jp);
+  attn_fwd_body<DH, true, QWG>(&tmQKV, &tmC, p, jp);
 }
 
 }  // namespace f5

@@ -48,19 +48,22 @@ struct AttnPlan {
   CUtensorMap tm;
   AttnParams p;
   dim3 grid;
-  int dh;  // head width: 64 or 128
+  int dh;   // head width: 64 or 128
+  int qwg;  // query warpgroups per CTA (64 qwg queries): 2, or 4 at dh 64
   // joint (MMDiT) attention: text segment
   int joint = 0;
   CUtensorMap tmC;
   AttnJointParams jp;
 };
+// qwg: query warpgroups per CTA, 2 or (dim_head 64) 4; 0 lets the planner choose from the grid (attn.cu).
 int attn_plan(AttnPlan* plan, const void* qkv, void* out, int batches, int seq, int heads, int dim_head,
-              const int* kv_len, float scale);
+              const int* kv_len, float scale, int qwg = 0);
 // Joint attention over [audio | text] keys for [audio | text] queries.  qkv_c fp16 [batches*seq_c, 3*inner], out_c
 // [batches*seq_c, inner]; c_len [batches] valid text keys (0 allowed) or null; text_q = 0 computes the audio queries
 // only (out_c is not written).
 int attn_joint_plan(AttnPlan* plan, const void* qkv, const void* qkv_c, void* out, void* out_c, int batches, int seq,
-                    int seq_c, int heads, int dim_head, const int* kv_len, const int* c_len, int text_q, float scale);
+                    int seq_c, int heads, int dim_head, const int* kv_len, const int* c_len, int text_q, float scale,
+                    int qwg = 0);
 int attn_run(const AttnPlan& plan, cudaStream_t s);
 
 // fp16 tensor map of rank 2 to 4, 128B swizzle: dims[0] is contiguous, strides[i] is the byte stride of dims[i + 1],

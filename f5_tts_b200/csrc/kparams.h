@@ -79,18 +79,25 @@ struct AttnJointParams {
   int seq_c;          // text tokens per sample
   const int* c_len;   // [Be] valid text keys per sample (0 allowed), or null (= seq_c)
   __half* out_c;      // [Be*seq_c, inner]
-  int q_blocks_a;     // audio query blocks, ceil(seq / kAttnBQ); grid.x beyond them are text query blocks
+  int q_blocks_a;     // audio query blocks, ceil(seq / (64 qwg)); grid.x beyond them are text query blocks
 };
 
-constexpr int kAttnThreads = 288;   // two softmax / MMA warpgroups (64 query rows each) + one TMA producer warp
-constexpr int kAttnBQ = 128;        // query rows per CTA
+// qwg softmax / MMA warpgroups (64 query rows each, 64 qwg query rows per CTA): qwg = 2, or 4 at head width 64
+// (attn.cu: attn_choose_qwg).  qwg = 2 adds a TMA producer warp.  qwg = 4 has none: 17 warps would put five warps on
+// one of the SM's four register-file quarters (16384 registers each) and cap every thread at 96 registers, where the
+// consumer spills; 16 warps leave it the 128 it needs, so consumer warp 0 issues the loads (attn.cuh).
+constexpr int attn_threads(int qwg) { return qwg == 4 ? 512 : 128 * qwg + 32; }
 constexpr int kAttnBKV = 128;       // keys per tile
 constexpr int kAttnStages = 3;      // K and V rings
 constexpr uint32_t kAttnTile = 128 * 64 * 2;  // 16 KB: one 128-row x 64-column TMA box
-// Q + K,V rings + alignment slack + barriers, for head width dh (dh / 64 boxes per tile).  dh = 128 with three stages
-// is 7 x 32 KB + 1.25 KB = 225.25 KB of the 227 KB an H100 CTA may have (DESIGN.md §4).
-constexpr size_t attn_smem_bytes(int dh) { return size_t(kAttnTile) * (dh / 64) * (1 + 2 * kAttnStages) + 1024 + 256; }
+// Q (qwg / 2 tiles of 128 rows) + K,V rings + alignment slack + barriers, for head width dh (dh / 64 boxes per tile).
+// dh = 128 with three stages is 7 x 32 KB + 1.25 KB = 225.25 KB of the 227 KB an H100 CTA may have (DESIGN.md §4);
+// dh = 64 at qwg = 4 is 8 x 16 KB + 1.25 KB.
+constexpr size_t attn_smem_bytes(int dh, int qwg = 2) {
+  return size_t(kAttnTile) * (dh / 64) * (qwg / 2 + 2 * kAttnStages) + 1024 + 256;
+}
 constexpr size_t kAttnSmem = attn_smem_bytes(64);
 static_assert(attn_smem_bytes(128) <= 227 * 1024, "dim_head 128 attention tiles exceed shared memory");
+static_assert(attn_smem_bytes(64, 4) <= 227 * 1024, "4-warpgroup attention tiles exceed shared memory");
 
 }  // namespace f5

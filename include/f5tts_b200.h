@@ -108,6 +108,17 @@ int f5_attention_joint(const void* qkv, const void* qkv_c, void* out, void* out_
                        int heads, int dim_head, const int* kv_len, const int* c_len, int text_q, float scale,
                        f5_stream_t stream);
 
+/* f5_attention_dh and f5_attention_joint with the query rows per CTA given: qwg consumer warpgroups of 64 rows, 2 or
+ * (dim_head 64) 4; anything else returns -1.  qwg = 0 is the planner's choice, which the two calls above always make.
+ * Both widths give the same output bit for bit; the choice only changes the grid (and so the speed). */
+int f5_attention_qwg(const void* qkv, void* out, int batches, int seq, int heads, int dim_head, const int* kv_len,
+                     float scale, int qwg, f5_stream_t stream);
+int f5_attention_joint_qwg(const void* qkv, const void* qkv_c, void* out, void* out_c, int batches, int seq, int seq_c,
+                           int heads, int dim_head, const int* kv_len, const int* c_len, int text_q, float scale,
+                           int qwg, f5_stream_t stream);
+/* the qwg that f5_attention_dh picks for this problem on the current device (-1 for invalid arguments) */
+int f5_attention_qwg_choice(int batches, int seq, int heads, int dim_head);
+
 /* Row normalisation + modulation -> fp16 (model/modules.py:312-326,333-347,753; x_transformers RMSNorm unett.py:154)
  *   mode 0: LN(eps) * (1 + a[c]) + b[c]   mode 1: LN(eps) * a[c] + b[c]   mode 2: x/||x|| * sqrt(D) * a[c] */
 int f5_row_norm(const float* x, void* out_f16, int rows, int D, int mode, float eps, const float* a, const float* b,
