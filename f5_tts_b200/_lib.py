@@ -212,11 +212,13 @@ EXPORTED_SYMBOLS = [
 ]
 
 # Test-only library: the same objects plus one extern "C" wrapper per kernel launcher (csrc/kernel_hooks.cu), used by
-# tests/test_gpu_small_kernels.py.  Nothing in the package loads it.
+# tests/test_gpu_small_kernels.py and tests/test_gpu_engine_kernels_f64.py.  Nothing in the package loads it.
 KERNELS_LIB_PATH = os.path.join(_HERE, "libf5tts_b200_kernels.so")
 KERNEL_HOOK_SYMBOLS = [
     "f5k_last_error", "f5k_row_norm", "f5k_dwconv7_ln", "f5k_text_gather", "f5k_mask_rows", "f5k_mask_rows_len",
     "f5k_grn_rows", "f5k_grn", "f5k_pack_input", "f5k_cfg_euler", "f5k_small_linear", "f5k_time_features",
     "f5k_silu_to_half", "f5k_rope_table", "f5k_prepend_time_token", "f5k_concat_half", "f5k_vocos_im2col",
     "f5k_ln_affine_f32", "f5k_istft", "f5k_row_norm_add_skip", "f5k_gemm_resid_sample",
+    "f5k_mmdit_text_embed", "f5k_text_avg_upsample", "f5k_row_norm_sample", "f5k_prepend_time_token_sample",
+    "f5k_dwconv7_ln_len", "f5k_vocos_im2col_len", "f5k_istft_len",
 ]

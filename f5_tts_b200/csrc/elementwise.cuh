@@ -235,13 +235,14 @@ __global__ void mmdit_text_embed_kernel(const long long* ids, int B, int nt, int
 // more for the last A % T tokens; rows at or past A, and every row when T == 0, are 0.  A = valid_len[b], or N.
 // grid (B, ceil(N / rows_per_block)); each block compacts the first K = min(nt, N) filler flags of its sample into
 // shared memory (positions at or past nt are always filler), then writes rows of both variants.
-// tx, out fp32 [2B, N, Td]; filler [B, N]; dynamic smem K ints.
+// tx, out fp32 [2B, N, Td]; filler [B, N]; dynamic smem 8 + K ints (the block's only shared memory).
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) text_avg_upsample_kernel(const float* tx, float* out, const uint8_t* filler,
                                                                 const int* valid_len, int B, int N, int K, int Td,
                                                                 int rows_per_block) {
-  extern __shared__ int vidx[];  // [K] positions of the valid text rows, in order
-  __shared__ int warp_cnt[8];
+  extern __shared__ int smem[];
+  int* warp_cnt = smem;  // [8] valid rows per warp in the current pass
+  int* vidx = smem + 8;  // [K] positions of the valid text rows, in order
   const int b = blockIdx.x;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   int T = 0;

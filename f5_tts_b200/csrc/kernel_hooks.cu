@@ -47,6 +47,25 @@ int f5k_row_norm(int mode, const float* x, void* out, int rows, int D, float eps
   return run_row_norm(mode, p, st(s));
 }
 
+// row norm mode 4 (f5_forward's per-sample AdaLN): mode 0 with scale / shift read at row
+// ((row / sample_seq) % samples) * step_stride of a and b
+int f5k_row_norm_sample(const float* x, void* out, int rows, int D, float eps, const float* a, const float* b,
+                        long long step_stride, int sample_seq, int samples, int params_static, void* s) {
+  NormParams p{};
+  p.x = x;
+  p.out = reinterpret_cast<__half*>(out);
+  p.rows = rows;
+  p.D = D;
+  p.eps = eps;
+  p.a = a;
+  p.b = b;
+  p.step_stride = step_stride;
+  p.params_static = params_static;
+  p.sample_seq = sample_seq;
+  p.samples = samples;
+  return run_row_norm(4, p, st(s));
+}
+
 // row norm mode 3: x += skip in place, out = RMSNorm(x) * g
 int f5k_row_norm_add_skip(float* x, const float* skip, void* out, int rows, int D, const float* g, void* s) {
   NormParams p{};
@@ -77,6 +96,24 @@ int f5k_dwconv7_ln(const float* x, void* out, int B, int N, int C, const float* 
   return run_dwconv7_ln(p, st(s));
 }
 
+// len: device int [B] rows of each sample (the Vocos decode of different-length mels)
+int f5k_dwconv7_ln_len(const float* x, void* out, int B, int N, int C, const float* w, const float* wb,
+                       const float* ln_w, const float* ln_b, float eps, const int* len, void* s) {
+  DwConvLnParams p{};
+  p.x = x;
+  p.out = reinterpret_cast<__half*>(out);
+  p.B = B;
+  p.N = N;
+  p.C = C;
+  p.w = w;
+  p.wb = wb;
+  p.ln_w = ln_w;
+  p.ln_b = ln_b;
+  p.eps = eps;
+  p.len = len;
+  return run_dwconv7_ln(p, st(s));
+}
+
 int f5k_text_gather(const long long* ids, int B, int nt, int N, int Td, const int* valid_len, const float* table,
                     int num_embeds, int add_pos, float* out, uint8_t* filler, void* s) {
   TextGatherParams p{};
@@ -92,6 +129,16 @@ int f5k_text_gather(const long long* ids, int B, int nt, int N, int Td, const in
   p.out = out;
   p.filler = filler;
   return run_text_gather(p, st(s));
+}
+
+int f5k_mmdit_text_embed(const long long* ids, int B, int Be, int nt, int D, const float* table, int num_embeds,
+                         int mask_padding, float* out, int* c_len, void* s) {
+  return run_mmdit_text_embed(ids, B, Be, nt, D, table, num_embeds, mask_padding, out, c_len, st(s));
+}
+
+int f5k_text_avg_upsample(const float* tx, float* out, const uint8_t* filler, const int* valid_len, int B, int N,
+                          int nt, int Td, void* s) {
+  return run_text_avg_upsample(tx, out, filler, valid_len, B, N, nt, Td, st(s));
 }
 
 int f5k_mask_rows(float* x, const uint8_t* filler, int BN, int rows, int C, void* s) {
@@ -166,12 +213,22 @@ int f5k_prepend_time_token(float* dst, const float* src, const float* t_emb, con
   return run_prepend_time_token(dst, src, t_emb, step_ptr, N, D, rows_out, st(s));
 }
 
+int f5k_prepend_time_token_sample(float* dst, const float* src, const float* t_emb, int samples, int N, int D,
+                                  long long rows_out, void* s) {
+  return run_prepend_time_token_per_sample(dst, src, t_emb, samples, N, D, rows_out, st(s));
+}
+
 int f5k_concat_half(const float* x, const float* skip, void* out, long long rows, int D, void* s) {
   return run_concat_half(x, skip, reinterpret_cast<__half*>(out), rows, D, st(s));
 }
 
 int f5k_vocos_im2col(const float* mel, int B, int C, int T, void* A, int Kpad, void* s) {
   return run_vocos_im2col(mel, B, C, T, reinterpret_cast<__half*>(A), Kpad, nullptr, st(s));
+}
+
+// lengths: device int [B] valid frames per sample
+int f5k_vocos_im2col_len(const float* mel, int B, int C, int T, void* A, int Kpad, const int* lengths, void* s) {
+  return run_vocos_im2col(mel, B, C, T, reinterpret_cast<__half*>(A), Kpad, lengths, st(s));
 }
 
 int f5k_ln_affine_f32(const float* x, float* out, int rows, int D, float eps, const float* w, const float* b, void* s) {
@@ -182,6 +239,12 @@ int f5k_istft(const float* head, int ld, float* frames, float* wav, int B, int T
   FftTables tab;
   if (int rc = fft_tables(&tab, st(s))) return rc;
   return run_istft(head, ld, frames, wav, B, T, nullptr, tab, st(s));
+}
+
+int f5k_istft_len(const float* head, int ld, float* frames, float* wav, int B, int T, const int* lengths, void* s) {
+  FftTables tab;
+  if (int rc = fft_tables(&tab, st(s))) return rc;
+  return run_istft(head, ld, frames, wav, B, T, lengths, tab, st(s));
 }
 
 }  // extern "C"

@@ -102,13 +102,15 @@ int run_mmdit_text_embed(const long long* ids, int B, int Be, int nt, int D, con
 int run_text_avg_upsample(const float* tx, float* out, const uint8_t* filler, const int* valid_len, int B, int N,
                           int nt, int Td, cudaStream_t s) {
   const int K = nt < N ? nt : N;
-  constexpr int kMaxTokens = 12288;  // the valid-row list of one sample in 48 KB of shared memory
+  // shared memory: the 8 warp counts and the valid-row list of one sample, within the 48 KB a block gets without an
+  // opt-in (12280 tokens)
+  constexpr int kMaxTokens = 48 * 1024 / (int)sizeof(int) - 8;
   if (K > kMaxTokens) {
     set_error("text average upsampling: at most %d text tokens per sample (got %d)", kMaxTokens, K);
     return -1;
   }
   constexpr int rows = 32;
-  text_avg_upsample_kernel<<<dim3(B, (N + rows - 1) / rows), 256, sizeof(int) * (K > 0 ? K : 1), s>>>(
+  text_avg_upsample_kernel<<<dim3(B, (N + rows - 1) / rows), 256, sizeof(int) * (8 + K), s>>>(
       tx, out, filler, valid_len, B, N, K, Td, rows);
   count_launch();
   return check_launch("text_avg_upsample_kernel");

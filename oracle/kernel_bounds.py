@@ -1,4 +1,5 @@
-"""float64 references of the GEMM epilogues and of attention, each with a per-element error bound for the sm_90a kernels.
+"""float64 references of the GEMM epilogues, of attention and of the bandwidth-bound kernels' row norms, positions and
+text embeddings, each with a per-element error bound for the sm_90a kernels.
 
 Pure torch: the references run on whichever device their inputs are on (the GPU tests keep them on the H100, the CPU
 test rehearses the bounds against an fp32 emulation of the kernels' arithmetic and against deliberately broken
@@ -15,6 +16,9 @@ from __future__ import annotations
 import math
 
 import torch
+import torch.nn.functional as F
+
+from oracle import f5_oracle as O
 
 U = 2.0 ** -24
 F64 = torch.float64
@@ -305,3 +309,118 @@ def attention_ref(q, k, v, kv_len=None, scale=None, block_kv=128):
     b4 = (36.0 + 2.0 * tiles) * U * o.abs()
     e = SLACK * (b1 + b2 + b3 + b4)
     return o, half_bound(o, e)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# bandwidth-bound kernels: row norms, depthwise conv, sinusoidal positions, text embeddings
+# ---------------------------------------------------------------------------------------------------------------------
+def gam(n):
+    return n * U / (1.0 - n * U)
+
+
+def ln_ref_bound(a, e_a, w, b, eps, depth):
+    """LayerNorm over the last axis of the exact pre-norm values `a` (float64), y = (a - mean) * rstd * w + b, and a
+    per-element bound on the kernel's fp32 y when its fp32 copy of `a` is off by at most `e_a`.
+
+    The kernel sums in fp32 with `depth` = terms per lane + 5 warp-shuffle levels:
+      mean:  e_mean = mean(e_a) + g(depth + 1) * mean|a|                  (sum of C terms, one division)
+      d:     e_d    = e_a + e_mean + u |d|                                (subtraction)
+      var:   e_var  = mean(2 |d| e_d + e_d^2) + g(depth + 2) * var        (squares, sum, division)
+      rstd:  rho    = (e_var / (var + eps) + u) / 2 + 4 u                 (relative; +eps, rsqrtf within 2 ulp)
+      y:     e_y    = |w| rstd (e_d + |d| rho) + 3 u |d rstd w| + u |y|   (two products, w itself rounded once, + b)
+    """
+    mean = a.mean(-1, keepdim=True)
+    d = a - mean
+    var = (d * d).mean(-1, keepdim=True)
+    rstd = (var + eps).rsqrt()
+    y = d * rstd * w + b
+    e_mean = e_a.mean(-1, keepdim=True) + gam(depth + 1) * a.abs().mean(-1, keepdim=True)
+    e_d = e_a + e_mean + U * d.abs()
+    e_var = (2 * d.abs() * e_d + e_d * e_d).mean(-1, keepdim=True) + gam(depth + 2) * var
+    rho = 0.5 * (e_var / (var + eps) + U) + 4 * U
+    e_y = w.abs() * rstd * (e_d + d.abs() * rho) + 3 * U * (d * rstd * w).abs() + U * y.abs()
+    return y, e_y
+
+
+def pos_bound(ang):
+    """cos / sin of ang = n * 10000^(-2i/dim), fp32: the exponent 2i/dim (u, times ln 1e4 < 9.3), powf (2 ulp = 4u), the
+    reciprocal (u) and the product n * freq (u) give |d ang| <= 16 u * ang; cosf / sinf add 2 ulp <= 4 u.  Bound used:
+    20 u * ang + 8 u."""
+    return 20 * U * ang + 8 * U
+
+
+def dwconv7_ref(x, w, wb):
+    """Depthwise Conv1d(k=7, pad=3) along the sequence of x [B, N, C] (float64), w [C, 7]; returns (a, sum|terms|)."""
+    B, N, C = x.shape
+    xp = F.pad(x, (0, 0, 3, 3))
+    a = wb.expand(B, N, C).clone()
+    s = wb.abs().expand(B, N, C).clone()
+    for t in range(7):
+        a = a + w[:, t] * xp[:, t:t + N]
+        s = s + (w[:, t] * xp[:, t:t + N]).abs()
+    return a, s
+
+
+def mmdit_text_embed_ref(table, ids, Be, mask_padding):
+    """(out, bound) of the MMDiT text embedding (backbones/mmdit.py:31-63) of ids [B, nt] (-1 padded) over the fp32
+    table [V + 1, D]; out [Be, nt, D] with Be = B (cond) or 2 B (cond, then uncond, whose ids are all 0):
+        out[v, b, n] = table[id + 1] + cat(cos, sin)(ang),   ang = min(n, 1023) * 10000^(-2i/D)
+    (precompute_freqs_cis(D, 1024), get_pos_embed_indices clamps at 1023), and 0 where the real text's id is -1 when
+    mask_padding, in both variants.  Bound: pos_bound(ang) for the fp32 angle and cosf / sinf, plus u |out| for the one
+    rounded addition; zeroed rows are exact (bound 0)."""
+    B, nt = ids.shape
+    D = table.shape[1]
+    dev = table.device
+    ids = ids.to(dev).long()
+    idx = torch.cat((ids + 1, torch.zeros_like(ids)), 0)[:Be]
+    freq = 10000.0 ** (-torch.arange(D // 2, dtype=F64, device=dev) * 2 / D)
+    a = torch.arange(nt, dtype=F64, device=dev).clamp(max=1023)[:, None] * freq[None]
+    out = table.to(F64)[idx] + torch.cat((a.cos(), a.sin()), -1)
+    keep = (ids != -1) if mask_padding else torch.ones_like(ids, dtype=torch.bool)
+    keep = torch.cat((keep, keep), 0)[:Be, :, None]
+    bound = pos_bound(torch.cat((a, a), -1)) + U * out.abs()
+    return torch.where(keep, out, 0.0), torch.where(keep, bound, 0.0)
+
+
+def avg_upsample_index(valid, audio_len, N):
+    """[B, N] source row of every output row of text average upsampling (backbones/dit.py:55-84), -1 where the row is 0.
+    Sample b's T valid text rows (the positions set in valid [B, K], in order) are spread over its first
+    A = min(audio_len[b], N) rows with dit.py's own loop: token j repeated A // T times, once more when
+    j >= T - A % T, cut at A.  Rows at or past A, and every row when T = 0, are 0.  Pure index arithmetic: the kernel's
+    copy of the selected rows must match bit for bit."""
+    B = valid.shape[0]
+    src = torch.full((B, N), -1, dtype=torch.long)
+    for b in range(B):
+        rows = torch.nonzero(valid[b].cpu()).flatten()
+        T, A = rows.numel(), min(int(audio_len[b]), N)
+        if T == 0 or A <= 0:
+            continue
+        base, rem = divmod(A, T)
+        reps = torch.tensor([base + (1 if j >= T - rem else 0) for j in range(T)], dtype=torch.long)
+        src[b, :A] = rows.repeat_interleave(reps)[:A]
+    return src
+
+
+def istft_ref(head, T):
+    """(wav, bound) of the Vocos ISTFT head (istft_frames + istft_ola) over head [B T, 1026] (log-magnitude | phase of
+    T >= 2 frames per sample, float64): the oracle's istft_center (== torch.istft(center=True)) of the spectrum
+    clipped at magnitude 100, wav [B, 256 (T - 1)].
+
+    Bound: per frame, A_t = (|X_0| + |X_512| + 2 sum_k |X_k|) / 1024 bounds |x_n|.  The input (expf, sincosf: 3 x 4 u)
+    and ten radix-2 stages (about 6 u each with table twiddles) put at most 100 u A_t on each frame sample; the window,
+    the <= 4-term overlap-add and the division by the envelope add 8 u of sum_t |w_n x_t,n| / env.  So
+    |d wav_i| <= (sum_t w_n (100 u A_t + 8 u |x_t,n|)) / env_i."""
+    nb = 513
+    B = head.shape[0] // T
+    mag = torch.exp(head[:, :nb]).clamp(max=100.0)
+    spec = torch.polar(mag, head[:, nb:]).view(B, T, nb).transpose(1, 2)  # [B, F, T]
+    win = torch.hann_window(1024, periodic=True, dtype=F64)
+    ref = O.istft_center(spec, window=win)
+    a = (mag[:, 0] + mag[:, nb - 1] + 2 * mag[:, 1:nb - 1].sum(-1)) / 1024  # [B T]
+    x = torch.fft.irfft(spec, n=1024, dim=1)  # [B, 1024, T]
+    per = win[None, :, None] * (100 * U * a.view(B, 1, T) + 8 * U * x.abs())
+    L = 1024 + 256 * (T - 1)
+    num = F.fold(per, output_size=(1, L), kernel_size=(1, 1024), stride=(1, 256))[:, 0, 0, 512:L - 512]
+    env = F.fold((win ** 2)[None, :, None].expand(1, 1024, T), output_size=(1, L), kernel_size=(1, 1024),
+                 stride=(1, 256))[:, 0, 0, 512:L - 512]
+    return ref, num / env

@@ -26,15 +26,12 @@ if not torch.cuda.is_available():
 
 from f5_tts_b200 import _lib, ops  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
-from oracle.kernel_bounds import assert_half, assert_within, ulp16  # noqa: E402,F401
+from oracle.kernel_bounds import (assert_half, assert_within, dwconv7_ref, gam, istft_ref,  # noqa: E402,F401
+                                  ln_ref_bound, pos_bound, ulp16)
 
 DEV = "cuda:0"
 U = 2.0 ** -24
 F64 = torch.float64
-
-
-def gam(n):
-    return n * U / (1.0 - n * U)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -96,49 +93,6 @@ def assert_equal(got, ref, what):
         d = torch.nonzero(got != ref)
         raise AssertionError(f"{what}: {d.shape[0]} elements differ, first at {d[0].tolist()}: "
                              f"got {got[tuple(d[0])].item()!r} ref {ref[tuple(d[0])].item()!r}")
-
-
-def ln_ref_bound(a, e_a, w, b, eps, depth):
-    """LayerNorm over the last axis of the exact pre-norm values `a` (float64), y = (a - mean) * rstd * w + b, and a
-    per-element bound on the kernel's fp32 y when its fp32 copy of `a` is off by at most `e_a`.
-
-    The kernel sums in fp32 with `depth` = terms per lane + 5 warp-shuffle levels:
-      mean:  e_mean = mean(e_a) + g(depth + 1) * mean|a|                  (sum of C terms, one division)
-      d:     e_d    = e_a + e_mean + u |d|                                (subtraction)
-      var:   e_var  = mean(2 |d| e_d + e_d^2) + g(depth + 2) * var        (squares, sum, division)
-      rstd:  rho    = (e_var / (var + eps) + u) / 2 + 4 u                 (relative; +eps, rsqrtf within 2 ulp)
-      y:     e_y    = |w| rstd (e_d + |d| rho) + 3 u |d rstd w| + u |y|   (two products, w itself rounded once, + b)
-    """
-    mean = a.mean(-1, keepdim=True)
-    d = a - mean
-    var = (d * d).mean(-1, keepdim=True)
-    rstd = (var + eps).rsqrt()
-    y = d * rstd * w + b
-    e_mean = e_a.mean(-1, keepdim=True) + gam(depth + 1) * a.abs().mean(-1, keepdim=True)
-    e_d = e_a + e_mean + U * d.abs()
-    e_var = (2 * d.abs() * e_d + e_d * e_d).mean(-1, keepdim=True) + gam(depth + 2) * var
-    rho = 0.5 * (e_var / (var + eps) + U) + 4 * U
-    e_y = w.abs() * rstd * (e_d + d.abs() * rho) + 3 * U * (d * rstd * w).abs() + U * y.abs()
-    return y, e_y
-
-
-def pos_bound(ang):
-    """cos / sin of ang = n * 10000^(-2i/dim), fp32: the exponent 2i/dim (u, times ln 1e4 < 9.3), powf (2 ulp = 4u), the
-    reciprocal (u) and the product n * freq (u) give |d ang| <= 16 u * ang; cosf / sinf add 2 ulp <= 4 u.  Bound used:
-    20 u * ang + 8 u."""
-    return 20 * U * ang + 8 * U
-
-
-def dwconv7_ref(x, w, wb):
-    """Depthwise Conv1d(k=7, pad=3) along the sequence of x [B, N, C] (float64), w [C, 7]; returns (a, sum|terms|)."""
-    B, N, C = x.shape
-    xp = F.pad(x, (0, 0, 3, 3))
-    a = wb.expand(B, N, C).clone()
-    s = wb.abs().expand(B, N, C).clone()
-    for t in range(7):
-        a = a + w[:, t] * xp[:, t:t + N]
-        s = s + (w[:, t] * xp[:, t:t + N]).abs()
-    return a, s
 
 
 def grn_ref(v, gamma, beta):
@@ -585,14 +539,9 @@ def test_vocos_im2col_ln(B, T):
 
 @pytest.mark.parametrize("B,T", VOCOS_CASES)
 def test_istft(B, T):
-    """run_istft (istft_frames + istft_ola) against the oracle's istft_center (== torch.istft(center=True)) in float64
-    of the clipped spectrum mag = min(exp(logmag), 100), with log-magnitudes above ln 100 and non-zero DC / Nyquist
-    phases (whose imaginary parts the inverse real FFT ignores).
-
-    Bound: per frame, A_t = (|X_0| + |X_512| + 2 sum_k |X_k|) / 1024 bounds |x_n|.  The input (expf, sincosf: 3 x 4 u)
-    and ten radix-2 stages (about 6 u each with table twiddles) put at most 100 u A_t on each frame sample; the window,
-    the <= 4-term overlap-add and the division by the envelope add 8 u of sum_t |w_n x_t,n| / env.  So
-    |d wav_i| <= (sum_t w_n (100 u A_t + 8 u |x_t,n|)) / env_i."""
+    """run_istft (istft_frames + istft_ola) against kernel_bounds.istft_ref: the oracle's istft_center in float64 of
+    the clipped spectrum mag = min(exp(logmag), 100), under istft_ref's bound, with log-magnitudes above ln 100 and
+    non-zero DC / Nyquist phases (whose imaginary parts the inverse real FFT ignores)."""
     ld, nb = 1026, 513
     g = torch.Generator().manual_seed(100 + T + B)
     logmag = torch.randn(B * T, nb, generator=g, dtype=F64) * 1.5 + 2.0
@@ -604,20 +553,9 @@ def test_istft(B, T):
     frames = torch.full((B * T, 1024), float("nan"), device=DEV)
     wav = torch.full((B, 256 * (T - 1)), float("nan"), device=DEV)
     launch("f5k_istft", head, ld, frames, wav, B, T)
-    h = head.cpu().double()
-    mag = torch.exp(h[:, :nb]).clamp(max=100.0)
-    spec = torch.polar(mag, h[:, nb:]).view(B, T, nb).transpose(1, 2)  # [B, F, T]
-    win = torch.hann_window(1024, periodic=True, dtype=F64)
-    ref = O.istft_center(spec, window=win)
+    ref, bound = istft_ref(head.cpu().double(), T)
     assert ref.shape == (B, 256 * (T - 1))
-    a = (mag[:, 0] + mag[:, nb - 1] + 2 * mag[:, 1:nb - 1].sum(-1)) / 1024  # [B T]
-    x = torch.fft.irfft(spec, n=1024, dim=1)  # [B, 1024, T]
-    per = win[None, :, None] * (100 * U * a.view(B, 1, T) + 8 * U * x.abs())
-    L = 1024 + 256 * (T - 1)
-    num = F.fold(per, output_size=(1, L), kernel_size=(1, 1024), stride=(1, 256))[:, 0, 0, 512:L - 512]
-    env = F.fold((win ** 2)[None, :, None].expand(1, 1024, T), output_size=(1, L), kernel_size=(1, 1024),
-                 stride=(1, 256))[:, 0, 0, 512:L - 512]
-    assert_within(wav.cpu(), ref, num / env, f"istft B{B} T{T}")
+    assert_within(wav.cpu(), ref, bound, f"istft B{B} T{T}")
 
 
 # ---------------------------------------------------------------------------------------------------------------------
