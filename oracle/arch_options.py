@@ -105,7 +105,7 @@ def dit_forward(sd, cfg, x, cond, text_emb, time, mask, cfg_infer: bool):
         mask = None if mask is None else torch.cat((mask, mask), dim=0)
     else:
         h = O.input_embedding(sd, x, cond, text_emb[0], False, mask)
-    ang = O.rope_angles(N, cfg.dim_head)
+    ang = O.rope_angles(N, cfg.dim_head, dtype=h.dtype)
     residual = h
     for i in range(cfg.depth):
         h = dit_block(sd, cfg, i, h, t_emb, mask, ang)
@@ -131,7 +131,7 @@ def unett_forward(sd, cfg, x, cond, text_emb, time, mask, cfg_infer: bool):
     h = torch.cat((t_emb[:, None], h), dim=1)
     if mask is not None:
         mask = F.pad(mask, (1, 0), value=True)
-    ang = O.rope_angles(N + 1, cfg.dim_head)
+    ang = O.rope_angles(N + 1, cfg.dim_head, dtype=h.dtype)
     skips = []
     half = cfg.depth // 2
     for i in range(cfg.depth):

@@ -81,26 +81,26 @@ def _ln_noaffine(x, eps=1e-6):
     return F.layer_norm(x, (x.shape[-1],), eps=eps)
 
 
-def sinus_time_features(t: torch.Tensor, dim=256, scale=1000.0) -> torch.Tensor:
-    """modules.py:157-169 — [B] -> [B, dim] = cat(sin, cos)"""
+def sinus_time_features(t: torch.Tensor, dim=256, scale=1000.0, dtype=torch.float32) -> torch.Tensor:
+    """modules.py:157-169 — [B] -> [B, dim] = cat(sin, cos), computed in `dtype`"""
     half = dim // 2
     k = math.log(10000.0) / (half - 1)
-    freqs = torch.exp(torch.arange(half, dtype=torch.float32) * -k)
-    arg = scale * t.float()[:, None] * freqs[None, :]
+    freqs = torch.exp(torch.arange(half, dtype=dtype) * -k)
+    arg = scale * t.to(dtype)[:, None] * freqs[None, :]
     return torch.cat((arg.sin(), arg.cos()), dim=-1)
 
 
 def timestep_embedding(sd, t: torch.Tensor, p="transformer.time_embed.") -> torch.Tensor:
-    """modules.py:852-862"""
-    h = sinus_time_features(t)
+    """modules.py:852-862, in the dtype of the time MLP's weights"""
+    h = sinus_time_features(t, dtype=sd[p + "time_mlp.0.weight"].dtype)
     h = _linear(sd, p + "time_mlp.0", h)
     return _linear(sd, p + "time_mlp.2", F.silu(h))
 
 
-def abs_pos_table(dim: int, end: int, theta=10000.0) -> torch.Tensor:
-    """modules.py:207-218 precompute_freqs_cis — [end, dim] = cat(cos, sin)"""
-    freqs = 1.0 / (theta ** (torch.arange(0, dim, 2)[: dim // 2].float() / dim))
-    ang = torch.outer(torch.arange(end).float(), freqs)
+def abs_pos_table(dim: int, end: int, theta=10000.0, dtype=torch.float32) -> torch.Tensor:
+    """modules.py:207-218 precompute_freqs_cis — [end, dim] = cat(cos, sin), computed in `dtype`"""
+    freqs = 1.0 / (theta ** (torch.arange(0, dim, 2)[: dim // 2].to(dtype) / dim))
+    ang = torch.outer(torch.arange(end).to(dtype), freqs)
     return torch.cat((ang.cos(), ang.sin()), dim=-1)
 
 
@@ -135,7 +135,7 @@ def text_embedding_dit(sd, cfg: ArchConfig, text, seq_len, drop_text: bool):
     if valid is not None:
         h = h.masked_fill(~valid[..., None], 0.0)
     if cfg.conv_layers > 0:
-        pos = abs_pos_table(cfg.tdim, n)
+        pos = abs_pos_table(cfg.tdim, n, dtype=h.dtype)
         if valid is not None:
             pos = pos[None] * valid[..., None].to(pos.dtype)
         h = h + pos
@@ -158,7 +158,7 @@ def text_embedding_unett(sd, cfg: ArchConfig, text, seq_len: int, drop_text: boo
         text = torch.zeros_like(text)
     h = F.embedding(text, sd[p + "text_embed.weight"])
     if cfg.conv_layers > 0:
-        h = h + abs_pos_table(cfg.tdim, 4096)[:seq_len]
+        h = h + abs_pos_table(cfg.tdim, 4096, dtype=h.dtype)[:seq_len]
         for i in range(cfg.conv_layers):
             if cfg.text_mask_padding:
                 h = h.masked_fill(filler[..., None], 0.0)
@@ -190,10 +190,11 @@ def input_embedding(sd, x, cond, text_emb, drop_audio_cond: bool, mask):
     return conv_position_embedding(sd, h, mask) + h
 
 
-def rope_angles(n: int, dim_head=64, base=10000.0) -> torch.Tensor:
-    """x_transformers RotaryEmbedding.forward_from_seq_len (dit.py:207,352): [n, dim_head], interleaved duplicate"""
-    inv = 1.0 / (base ** (torch.arange(0, dim_head, 2).float() / dim_head))
-    ang = torch.outer(torch.arange(n).float(), inv)
+def rope_angles(n: int, dim_head=64, base=10000.0, dtype=torch.float32) -> torch.Tensor:
+    """x_transformers RotaryEmbedding.forward_from_seq_len (dit.py:207,352): [n, dim_head], interleaved duplicate,
+    computed in `dtype`"""
+    inv = 1.0 / (base ** (torch.arange(0, dim_head, 2).to(dtype) / dim_head))
+    ang = torch.outer(torch.arange(n).to(dtype), inv)
     return torch.stack((ang, ang), dim=-1).flatten(-2)
 
 
@@ -262,7 +263,7 @@ def dit_forward(sd, cfg: ArchConfig, x, cond, text_emb, time, mask, cfg_infer: b
         mask = None if mask is None else torch.cat((mask, mask), dim=0)
     else:
         h = input_embedding(sd, x, cond, text_emb[0], False, mask)
-    ang = rope_angles(N, cfg.dim_head)
+    ang = rope_angles(N, cfg.dim_head, dtype=h.dtype)
     for i in range(cfg.depth):
         h = dit_block(sd, cfg, i, h, t_emb, mask, ang)
     mod = _linear(sd, "transformer.norm_out.linear", F.silu(t_emb))  # modules.py:342-347
@@ -290,7 +291,7 @@ def unett_forward(sd, cfg: ArchConfig, x, cond, text_emb, time, mask, cfg_infer:
     h = torch.cat((t_emb[:, None], h), dim=1)
     if mask is not None:
         mask = F.pad(mask, (1, 0), value=True)
-    ang = rope_angles(N + 1, cfg.dim_head)
+    ang = rope_angles(N + 1, cfg.dim_head, dtype=h.dtype)
     skips = []
     half = cfg.depth // 2
     for i in range(cfg.depth):

@@ -27,7 +27,7 @@ def text_embedding(sd, cfg, text, drop_text: bool):
         ids = torch.zeros_like(ids)
     h = sd[P + "text_embed.text_embed.weight"][ids]
     pos = torch.arange(text.shape[1]).clamp(max=1023)  # get_pos_embed_indices, modules.py:221-230
-    h = h + O.abs_pos_table(cfg.dim, 1024)[pos]
+    h = h + O.abs_pos_table(cfg.dim, 1024, dtype=h.dtype)[pos]
     if cfg.text_mask_padding:
         h = h.masked_fill(pad[..., None], 0.0)
     return h
@@ -46,7 +46,7 @@ def _heads(sd, cfg, p, x, names, norms):
     q, k, v = (O._linear(sd, p + nm, x).view(B, n, cfg.heads, cfg.dim_head).transpose(1, 2) for nm in names)
     if cfg.qk_norm == "rms_norm":
         q, k = OA.rms_norm(q, sd[p + norms[0]]), OA.rms_norm(k, sd[p + norms[1]])
-    ang = O.rope_angles(n, cfg.dim_head)  # every head, positions 0.. per stream
+    ang = O.rope_angles(n, cfg.dim_head, dtype=x.dtype)  # every head, positions 0.. per stream
     return O.apply_rope(q, ang), O.apply_rope(k, ang), v
 
 

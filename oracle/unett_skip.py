@@ -33,7 +33,7 @@ def unett_forward(sd, cfg, x, cond, text_emb, time, mask, cfg_infer: bool):
     h = torch.cat((t_emb[:, None], h), dim=1)
     if mask is not None:
         mask = F.pad(mask, (1, 0), value=True)
-    ang = O.rope_angles(N + 1, cfg.dim_head)
+    ang = O.rope_angles(N + 1, cfg.dim_head, dtype=h.dtype)
     skips = []
     half = cfg.depth // 2
     for i in range(cfg.depth):

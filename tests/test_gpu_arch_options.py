@@ -31,6 +31,7 @@ from oracle import arch_options as OA  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
 from oracle import make_golden as MG  # noqa: E402
 from oracle import make_golden_arch_options as MA  # noqa: E402
+from oracle import step_increment as SI  # noqa: E402
 
 DEV = "cuda:0"
 TOL = 5e-3
@@ -175,6 +176,7 @@ def test_sample_vs_reference_fixture(golden_dir, name):
     finally:
         model.odeint_kwargs = dict(method="euler")
     assert traj.shape[0] == int(z["steps"]) + 1 and out.shape == z["out"].shape
+    SI.check(traj[1], z["y0"], z["traj_1"], z["duration"] if cfg.attn_mask_enabled else None, name)
     r1, rn = rel(traj[1], z["traj_1"]), rel(out, z["out"])
     print(f"[{name}] step-1 rel-L2 {r1:.3e}  final rel-L2 {rn:.3e}")
     assert r1 <= TOL and rn <= TOL

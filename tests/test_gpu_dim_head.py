@@ -26,6 +26,7 @@ from f5_tts_b200.ops import EPI_QKV_NORM_ROPE, EPI_QKV_ROPE  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
 from oracle import make_golden as MG  # noqa: E402
 from oracle import make_golden_dim_head as MD  # noqa: E402
+from oracle import step_increment as SI  # noqa: E402
 
 DEV = "cuda:0"
 TOL = 5e-3
@@ -212,6 +213,7 @@ def test_sample_vs_reference_fixture(golden_dir, name):
     finally:
         model.odeint_kwargs = dict(method="euler")
     assert traj.shape[0] == int(z["steps"]) + 1 and out.shape == z["out"].shape
+    SI.check(traj[1], z["y0"], z["traj_1"], z["duration"] if cfg.attn_mask_enabled else None, name)
     r1, rn = rel(traj[1], z["traj_1"]), rel(out, z["out"])
     print(f"[{name}] step-1 rel-L2 {r1:.3e}  final rel-L2 {rn:.3e}")
     assert r1 <= TOL and rn <= TOL

@@ -29,6 +29,7 @@ if not torch.cuda.is_available():
 import f5_tts_b200 as F5  # noqa: E402
 import synthdata as SD  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
+from oracle import step_increment as SI  # noqa: E402
 
 DEV = "cuda:0"
 TOL = 5e-3
@@ -65,6 +66,7 @@ def test_cfg2_full_nfe32_vs_reference(golden_dir):
     out, traj = model.sample(wav.to(DEV), text.to(DEV), int(duration[0]), steps=int(z["steps"]),
                              cfg_strength=float(z["cfg_strength"]), sway_sampling_coef=float(z["sway"]), seed=int(z["seed"]),
                              y0=torch.from_numpy(z["y0"]).to(DEV))
+    SI.check(traj[1], z["y0"], z["traj_1"], None, "cfg2_full_nfe32")  # every row: B = 1, no mask
     n_ref = int(z["n_ref"])
     gen = slice(n_ref, None)
     drift = {int(k): rel(traj[int(k)][:, gen], torch.from_numpy(z[f"traj_{int(k)}"])[:, gen]) for k in z["kept"]}
@@ -98,15 +100,19 @@ def _golden_vs_gpu(name, golden_dir):
                              cfg_strength=SD.CFG_STRENGTH, sway_sampling_coef=SD.SWAY, seed=int(z["seed"]), y0=y0.to(DEV))
     g1, gN = torch.from_numpy(z["step1"]), torch.from_numpy(z["final"])
     worst, at = 0.0, 0
+    inc = ([], [], [])  # the first increment's rows: engine, y0, fixture
     for b in range(w["B"]):  # every `stride`-th valid generated row of each utterance
         sl = slice(int(lens[b]), int(duration[b]), stride)
         n = len(range(*sl.indices(int(duration[b]))))
+        for rows, t in zip(inc, (traj[1][b, sl], y0[b, sl], g1[at: at + n])):
+            rows.append(t)
         r1 = rel(traj[1][b, sl], g1[at: at + n])
         rN = rel(out[b, sl], gN[at: at + n])
         at += n
         worst = max(worst, r1, rN)
         print(f"[{name}] utt {b} frames {int(duration[b])}: step-1 {r1:.3e}  final({steps} steps) {rN:.3e}")
     assert at == g1.shape[0] == gN.shape[0]
+    SI.check_rows(*inc, tag=f"fullsize_{name}")
     assert worst <= TOL
     return worst
 

@@ -25,6 +25,7 @@ import synthdata as SD  # noqa: E402
 from f5_tts_b200 import _lib  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
 from oracle import ode_midpoint as OM  # noqa: E402
+from oracle import step_increment as SI  # noqa: E402
 
 DEV = "cuda:0"
 TOL = 5e-3
@@ -65,6 +66,7 @@ def test_midpoint_vs_reference_golden(golden_dir):
     model = with_method(build(cfg, wseed)[0], "midpoint")
     out, traj = model.sample(cond.to(DEV), text.to(DEV), dur.to(DEV), lens=lens.to(DEV), **kw,
                              y0=torch.from_numpy(z["y0"]).to(DEV))
+    SI.check(traj[1], z["y0"], z["traj_1"], None, MM.FULL)
     r1, rN = rel(traj[1], torch.from_numpy(z["traj_1"])), rel(out, torch.from_numpy(z["out"]))
     print(f"[midpoint golden] step-1 rel-L2 {r1:.3e}  final rel-L2 {rN:.3e}")
     assert traj.shape[0] == kw["steps"] + 1 and out.shape == z["out"].shape

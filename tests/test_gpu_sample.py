@@ -20,6 +20,7 @@ if not torch.cuda.is_available():
 
 import f5_tts_b200 as F5  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
+from oracle import step_increment as SI  # noqa: E402
 
 DEV = "cuda:0"
 TOL = 5e-3
@@ -63,6 +64,7 @@ def test_sample_vs_reference_golden(golden_dir, name):
                              duration=duration, lens=lens, steps=int(z["steps"]), cfg_strength=float(z["cfg_strength"]),
                              sway_sampling_coef=float(z["sway"]), seed=int(z["seed"]),
                              y0=torch.from_numpy(z["y0"]).to(DEV))
+    SI.check(traj[1], z["y0"], z["traj_1"], z["duration"] if cfg.attn_mask_enabled else None, name)
     r1, rN = rel(traj[1], torch.from_numpy(z["traj_1"])), rel(out, torch.from_numpy(z["out"]))
     print(f"[{name}] step-1 rel-L2 {r1:.3e}  final rel-L2 {rN:.3e}")
     assert traj.shape[0] == int(z["steps"]) + 1 and out.shape == z["out"].shape

@@ -30,6 +30,7 @@ from f5_tts_b200 import _lib, api, infer, ops  # noqa: E402
 from f5_tts_b200.model import list_str_to_idx  # noqa: E402
 from oracle import f5_oracle as O  # noqa: E402
 from oracle import ode_midpoint as OM  # noqa: E402
+from oracle import step_increment as SI  # noqa: E402
 
 DEV = "cuda:0"
 TOL = 5e-3
@@ -180,6 +181,7 @@ def test_sample_vs_reference_fixture(golden_dir, name):
                              duration=duration, lens=lens, steps=int(z["steps"]), cfg_strength=float(z["cfg_strength"]),
                              sway_sampling_coef=sway, seed=int(z["seed"]), y0=torch.from_numpy(z["y0"]).to(DEV))
     assert traj.shape[0] == int(z["steps"]) + 1 and out.shape == z["out"].shape
+    SI.check(traj[1], z["y0"], z["traj_1"], z["duration"] if cfg.attn_mask_enabled else None, name)
     want, want1, t1 = torch.from_numpy(z["out"]), torch.from_numpy(z["traj_1"]), traj[1]
     if cfg.attn_mask_enabled:  # key-masked mode: padded rows are not computed, compare every sample's valid rows
         durs = z["duration"].tolist()
