@@ -3,7 +3,8 @@
 Same constructor / ``infer`` signature and return value ``(wav np.float32[nw], sr, spec np[100, n])``.  Differences,
 all forced by the offline image and the scope of this build: model configs are the six shipped architectures
 (Base and Small of F5TTS_v1, F5TTS and E2TTS) hard-coded below (hydra/omegaconf are not installed; values copied from configs/*.yaml ``model.arch``); checkpoints
-and the vocoder must be given as local paths (no network); ``transcribe`` and silence removal are not mirrored.
+and the vocoder must be given as local paths (no network); ``transcribe`` is not mirrored.  ``remove_silence`` trims
+the written file as the reference does; the returned array stays untrimmed.
 """
 from __future__ import annotations
 
@@ -36,6 +37,9 @@ MODEL_ARCH = {
     "E2TTS_Small": (UNetT, dict(dim=768, depth=20, heads=12, ff_mult=4, text_mask_padding=False, pe_attn_head=1)),
 }
 
+CKPT_REQUIRED = ("ckpt_file is required: there is no network here to fetch hf://SWivid/... "
+                 "(api.py:65-81 in the reference downloads it)")
+
 
 def seed_everything(seed=0):
     """model/utils.py:19-26"""
@@ -61,8 +65,7 @@ class F5TTS:
         self.vocoder = _infer.load_vocoder(self.mel_spec_type, vocoder_local_path is not None, vocoder_local_path,
                                            self.device, hf_cache_dir)
         if not ckpt_file:
-            raise FileNotFoundError("ckpt_file is required: there is no network here to fetch hf://SWivid/... "
-                                    "(api.py:65-81 in the reference downloads it)")
+            raise FileNotFoundError(CKPT_REQUIRED)
         self.ema_model = _infer.load_model(model_cls, model_arc, ckpt_file, self.mel_spec_type, vocab_file,
                                            self.ode_method, self.use_ema, self.device,
                                            cfg_parallel_device=cfg_parallel_device,
@@ -70,14 +73,10 @@ class F5TTS:
         self.seed = None
 
     def export_wav(self, wav, file_wave, remove_silence=False):
-        import wave
-
-        pcm = (np.clip(np.asarray(wav), -1.0, 1.0) * 32767.0).astype("<i2")
-        with wave.open(file_wave, "wb") as f:
-            f.setnchannels(1)
-            f.setsampwidth(2)
-            f.setframerate(self.target_sample_rate)
-            f.writeframes(pcm.tobytes())
+        """api.py:89-93: 16-bit PCM wav; `remove_silence` trims the written file (`infer.remove_silence_for_generated_wav`)."""
+        _infer._write_wav(file_wave, wav, self.target_sample_rate)
+        if remove_silence:
+            _infer.remove_silence_for_generated_wav(file_wave)
 
     def export_spectrogram(self, spec, file_spec):
         np.save(file_spec, spec)

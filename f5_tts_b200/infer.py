@@ -4,8 +4,10 @@ functions on (or feeding) the hot path: same names, arguments, defaults and retu
 Reference anchors (relative to /root/reference/src/f5_tts/infer/utils_infer.py):
   module constants 52-65 · chunk_text 73-102 · load_vocoder 106-145 · load_checkpoint 190-232 · load_model 238-276 ·
   infer_process 384-434 · infer_batch_process 440-593 (``_infer_basic`` 477-520).
-Out of scope here (SURVEY.md §2 rows 7, 10-12): ASR transcription, pydub silence trimming, matplotlib spectrogram
-dumps, BigVGAN.  ``preprocess_ref_audio_text`` keeps only the text normalisation of utils_infer.py:369-376.
+  remove_silence_for_generated_wav 599-608.
+Out of scope here (SURVEY.md §2 rows 7, 10-12): ASR transcription, the pydub clipping of the reference audio,
+matplotlib spectrogram dumps, BigVGAN.  ``preprocess_ref_audio_text`` keeps only the text normalisation of
+utils_infer.py:369-376.
 """
 from __future__ import annotations
 
@@ -249,6 +251,132 @@ def _load_wav(path):
         raise NotImplementedError("only 16-bit PCM wav is read natively")
     data = np.frombuffer(raw, dtype="<i2").astype(np.float32) / 32768.0
     return torch.from_numpy(data.reshape(-1, ch).T.copy()), sr
+
+
+def _write_wav(path, wav, sample_rate=target_sample_rate):
+    """Mono 16-bit PCM wav of a float waveform: clipped to [-1, 1], scaled by 32767 and truncated toward zero."""
+    pcm = (np.clip(np.asarray(wav), -1.0, 1.0) * 32767.0).astype("<i2")
+    with wave.open(path, "wb") as f:
+        f.setnchannels(1)
+        f.setsampwidth(2)
+        f.setframerate(sample_rate)
+        f.writeframes(pcm.tobytes())
+
+
+# ------------------------------------------------------------------------------------------------ silence removal
+def _ms_to_frame(ms, rate):
+    """pydub's millisecond -> frame position (AudioSegment._parse_position: int(frame_count(ms=ms)))."""
+    return (np.asarray(ms, dtype=np.float64) * (rate / 1000.0)).astype(np.int64)
+
+
+def _pydub_len(n_frames, rate):
+    """len(AudioSegment) in milliseconds: round(1000 * frames / rate), Python's round (half to even)."""
+    return round(1000 * (float(n_frames) / rate))
+
+
+def _slice_frames(pcm, rate, start_ms, end_ms):
+    """AudioSegment[start_ms:end_ms] on [n, channels] int16 frames.  Both ends are clamped to len(segment); an end
+    that the millisecond rounding puts past the last frame is filled with zero frames, as pydub does, unless the slice
+    is empty."""
+    seg_len = _pydub_len(len(pcm), rate)
+    fs, fe = (int(v) for v in _ms_to_frame([min(start_ms, seg_len), min(end_ms, seg_len)], rate))
+    data = pcm[fs:fe]
+    if 0 < len(data) < fe - fs:
+        data = np.concatenate([data, np.zeros((fe - fs - len(data), pcm.shape[1]), pcm.dtype)])
+    return data
+
+
+def _silence_window_rms(pcm, rate, min_silence_len=1000, seek_step=10):
+    """(window starts in ms, audioop.rms of each window) for pydub's `detect_silence` scan: windows of
+    `min_silence_len` ms every `seek_step` ms, plus a final window ending at len(segment) when the steps miss it.
+
+    The RMS is audioop.rms's: the integer part of sqrt(sum of squares / samples) over every sample of every channel
+    in the window, zero for an empty window.  The sums come from int64 prefix sums of squares, so the scan is O(n);
+    they convert to float64 exactly while a window has fewer than 2**23 samples, as audioop's double accumulator
+    does."""
+    seg_len = _pydub_len(len(pcm), rate)
+    last = seg_len - min_silence_len
+    starts = list(range(0, last + 1, seek_step))
+    if last % seek_step:
+        starts.append(last)
+    sq = np.square(pcm.astype(np.int64)).sum(axis=1)
+    prefix = np.concatenate([np.zeros(1, np.int64), np.cumsum(sq)])
+    s = np.asarray(starts, dtype=np.int64)
+    fs = _ms_to_frame(np.minimum(s, seg_len), rate)
+    fe = _ms_to_frame(np.minimum(s + min_silence_len, seg_len), rate)
+    n = len(pcm)
+    lo, hi = np.minimum(fs, n), np.minimum(fe, n)
+    frames = np.where(hi > lo, np.maximum(fe - fs, 0), 0)  # zero-filled ends count as samples (_slice_frames)
+    total = (prefix[hi] - prefix[lo]).astype(np.float64)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        rms = np.where(frames > 0, np.floor(np.sqrt(total / (frames * pcm.shape[1]))), 0.0)
+    return starts, rms.astype(np.int64)
+
+
+def _split_on_silence(pcm, rate, min_silence_len=1000, silence_thresh=-50, keep_silence=500, seek_step=10):
+    """pydub.silence.split_on_silence on [n, channels] int16 frames: the list of kept [m, channels] pieces.
+
+    Restated from pydub 0.25's published `detect_silence` / `detect_nonsilent` / `split_on_silence` (pydub is not a
+    dependency of this package): a window is silent when its RMS is at most db_to_float(silence_thresh) * 32768; consecutive silent
+    windows merge into ranges; the non-silent ranges between them are padded by `keep_silence` ms each way, and two
+    padded ranges that overlap are split at their midpoint."""
+    seg_len = _pydub_len(len(pcm), rate)
+    silent = []
+    if seg_len >= min_silence_len:
+        thresh = 10 ** (float(silence_thresh) / 20) * 32768.0
+        starts, rms = _silence_window_rms(pcm, rate, min_silence_len, seek_step)
+        silence_starts = [i for i, r in zip(starts, rms) if r <= thresh]
+        if silence_starts:
+            prev = cur = silence_starts[0]
+            for i in silence_starts[1:]:
+                if i != prev + seek_step and i > prev + min_silence_len:
+                    silent.append([cur, prev + min_silence_len])
+                    cur = i
+                prev = i
+            silent.append([cur, prev + min_silence_len])
+    if not silent:
+        nonsilent = [[0, seg_len]]
+    elif silent[0] == [0, seg_len]:
+        nonsilent = []
+    else:
+        nonsilent, prev_end = [], 0
+        for start, end in silent:
+            nonsilent.append([prev_end, start])
+            prev_end = end
+        if silent[-1][1] != seg_len:
+            nonsilent.append([prev_end, seg_len])
+        if nonsilent[0] == [0, 0]:
+            nonsilent.pop(0)
+    ranges = [[start - keep_silence, end + keep_silence] for start, end in nonsilent]
+    for a, b in zip(ranges, ranges[1:]):
+        if b[0] < a[1]:
+            a[1] = (a[1] + b[0]) // 2
+            b[0] = a[1]
+    return [_slice_frames(pcm, rate, max(start, 0), min(end, seg_len)) for start, end in ranges]
+
+
+def remove_silence_for_generated_wav(filename):
+    """utils_infer.py:599-608: cut every silence of 1 s or more in a 16-bit wav down to 0.5 s on each side, in place.
+
+    The reference runs pydub's split_on_silence(min_silence_len=1000, silence_thresh=-50, keep_silence=500,
+    seek_step=10), concatenates the pieces and writes the file back.  pydub is not a dependency here, so its loop logic
+    (window placement, range merging, padding, midpoint split, millisecond-to-frame rounding) is restated in
+    `_split_on_silence`; the window RMS is pinned against `audioop.rms` itself, window by window.  The file keeps its
+    rate, channel count and width.  (pydub concatenates onto an empty 11025 Hz segment, so it would write a result at
+    11025 Hz when the input rate is lower or every piece is dropped.)"""
+    with wave.open(filename, "rb") as f:
+        rate, ch, width = f.getframerate(), f.getnchannels(), f.getsampwidth()
+        raw = f.readframes(f.getnframes())
+    if width != 2:
+        raise NotImplementedError("only 16-bit PCM wav is read natively")
+    pcm = np.frombuffer(raw, dtype="<i2").reshape(-1, ch)
+    pieces = _split_on_silence(pcm, rate)
+    out = np.concatenate(pieces) if pieces else pcm[:0]
+    with wave.open(filename, "wb") as f:
+        f.setnchannels(ch)
+        f.setsampwidth(2)
+        f.setframerate(rate)
+        f.writeframes(out.astype("<i2").tobytes())
 
 
 # ------------------------------------------------------------------------------------------------ inference
